@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- log lines/sec through the B200 detector (BASELINE.json metric).
+"""bench.py -- log lines/sec through the H100 detector (BASELINE.json metric).
 
 Workload (BASELINE config 2 shape, windows as in config 4): every GPU owns 17 synthetic messages of
-65 536 audit records x 256 B (16 MiB each, 272 MiB > the 126 MB L2).  Message 0 is the anomaly-free
+65 536 audit records x 256 B (16 MiB each, 272 MiB > the 50 MB L2).  Message 0 is the anomaly-free
 training window (untimed).  A STEP is one WINDOW of 8 consecutive detection messages (512k records,
 128 MiB) and, with more than one GPU, ONE NCCL sum-all-reduce of the window's statistics
 (SURVEY.md 8d, config 4); the timed steps cycle over the 16 detection messages.  Multi-GPU: the
@@ -17,6 +17,9 @@ stream shards by message across ranks (weak scaling), no data-path collective.
   roofline  the tokenizer+detector kernel (one launch per message): algorithmic bytes per launch
             (record bytes + 1 B flag + 4 B score per record) / average launch duration over the
             timed region, against MEASURED_PEAKS.json.
+  --dump-outputs DIR  after the timed steps: flags.npy / scores.npy (float32, one row per message of the
+            last timed step) = what the detector returned for those messages; inputs are seeded, so two builds
+            can be compared output for output.
   cpu_baseline  rank 0, N=1: the oracle's C restatement on all host cores (pinned pthreads, median
             of 5 x 2 s) and, as `reference_engine`, the reference's OWN Engine/Service per record.
   extra.configs  BASELINE configs 3 (through NNG-framed sockets), 4 (windows; = this run) and 5
@@ -68,15 +71,15 @@ def _peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM, HBM3 3.35 TB/s)"
 
 
 KERNEL_SOURCES = ("dm_kernels_stream.cuh", "dm_kernels_index.cuh", "dm_device.cuh", "dm_hash.h")
 
 
 def _csrc_sha() -> str:
-    """Fingerprint of the sources of the dominant kernel (dm_k_stream and what it includes): ties the ncu numbers under
-    profiles/ to the code they were taken on."""
+    """Fingerprint of the sources of the dominant kernel (dm_k_stream and what it includes): ties a bench line to the
+    code it was taken on."""
     h = hashlib.sha256()
     d = os.path.join(ROOT, "detectmateservice_b200", "csrc")
     for f in KERNEL_SOURCES:
@@ -103,6 +106,7 @@ class ClockSampler(threading.Thread):
         self.index, self.period = index, period
         self.samples, self.reasons = [], set()
         self.max_mhz = None
+        self.gpu_name, self.power_limit_w = None, None
         self._halt = threading.Event()
         self.ok = False
         try:
@@ -111,6 +115,8 @@ class ClockSampler(threading.Thread):
             self.nv = pynvml
             self.h = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM)
+            self.gpu_name = pynvml.nvmlDeviceGetName(self.h)
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
             self.ok = True
         except Exception:
             self.nv = None
@@ -143,8 +149,9 @@ class ClockSampler(threading.Thread):
         if self.is_alive():
             self.join(timeout=2)
         med = float(np.median(self.samples)) if self.samples else None
-        return {"sm_mhz": med, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons),
-                "samples": len(self.samples)}
+        name = self.gpu_name.decode() if isinstance(self.gpu_name, bytes) else self.gpu_name
+        return {"gpu": name, "power_limit_w": self.power_limit_w, "sm_mhz": med, "sm_max_mhz": self.max_mhz,
+                "reasons": sorted(self.reasons), "samples": len(self.samples)}
 
 
 # ------------------------------------------------------------------------------------------
@@ -165,7 +172,7 @@ def _reference_engine_leg(msgs, seconds: float = 4.0):
     from detectmateservice_b200.synth import MONITORED_KEYS
     from oracle import ref_engine, rtok
     if ref_engine.reference_path() is None:
-        return {"unavailable": "reference service neither in baseline/_ref nor in /root/reference/src"}
+        return {"unavailable": "the reference service is not in oracle/_ref (make -C oracle ref)"}
     train = rtok.split_records(msgs[0][:LINE_BYTES * 2000])
     # (anomaly-free records: an alert would be answered on the feeder's socket)
     detect = rtok.split_records(msgs[0][LINE_BYTES * 2000:LINE_BYTES * 6000])
@@ -284,6 +291,20 @@ def _config3_engine(h_msgs, nbytes, device: int, seconds: float = 2.0):
     return res
 
 
+def _dump_outputs(out_dir: str, rank: int, world: int, last_step: int, n_lines_msg, out_flags, out_scores):
+    """flags.npy / scores.npy (float32, WINDOW_MSGS x records): the outputs of the messages of the last timed step, in
+    window order (message 1 + ((last_step * WINDOW_MSGS + m) % N_DETECT) in row m).  With more than one GPU every
+    rank writes its own pair, suffixed _rank<r>."""
+    import torch
+    torch.cuda.synchronize()
+    n = [n_lines_msg[1 + ((last_step * WINDOW_MSGS + m) % N_DETECT)] for m in range(WINDOW_MSGS)]
+    assert len(set(n)) == 1, "the messages of a window have the same number of records"
+    sfx = f"_rank{rank}" if world > 1 else ""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"flags{sfx}.npy"), out_flags[:, :n[0]].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, f"scores{sfx}.npy"), out_scores[:, :n[0]].cpu().numpy().astype(np.float32))
+
+
 def run_gpu(args):
     import torch
     import torch.distributed as dist
@@ -335,8 +356,12 @@ def run_gpu(args):
     for hp in h_msgs:
         _lib.check(_lib.load().dm_host_cache_flush(hp.data_ptr(), hp.numel()))
     cap = LINES_PER_MSG + 16
-    d_flags = torch.zeros(cap, dtype=torch.uint8, device=dev)
-    d_scores = torch.zeros(cap, dtype=torch.float32, device=dev)
+    # every message of a window has its own output rows, as a caller that keeps a window's results needs
+    # (row stride rounded up to 256 B)
+    stride = (cap + 255) & ~255
+    out_flags = torch.zeros((WINDOW_MSGS, stride), dtype=torch.uint8, device=dev)
+    out_scores = torch.zeros((WINDOW_MSGS, stride), dtype=torch.float32, device=dev)
+    d_flags, d_scores = out_flags[0], out_scores[0]
     from detectmateservice_b200.window import DeviceWindow
     dwin = DeviceWindow(det, rank, world, dev)
     if world > 1 and os.environ.get("DM_WINDOW", "native") == "native":
@@ -372,7 +397,7 @@ def run_gpu(args):
         n = 0
         for m in range(WINDOW_MSGS):
             j = 1 + ((i * WINDOW_MSGS + m) % N_DETECT)
-            det.enqueue_device(d_msgs[j].data_ptr(), nbytes[j], 0, d_flags.data_ptr(), d_scores.data_ptr(), cap, sp)
+            det.enqueue_device(d_msgs[j].data_ptr(), nbytes[j], 0, out_flags[m].data_ptr(), out_scores[m].data_ptr(), cap, sp)
             n += n_lines_msg[j]
         if world > 1:
             window(False)
@@ -402,6 +427,8 @@ def run_gpu(args):
     barrier()
     ms = e0.elapsed_time(e1)
     _, _, launches1 = det.profile_read()
+    if args.dump_outputs:
+        _dump_outputs(args.dump_outputs, rank, world, args.steps - 1, n_lines_msg, out_flags, out_scores)
     t = torch.tensor([ms], dtype=torch.float64, device=dev)
     tot = torch.tensor([float(lines_timed)], dtype=torch.float64, device=dev)
     if world > 1:
@@ -438,19 +465,8 @@ def run_gpu(args):
     det.set_overlap(True)
     peak, peak_src = _peaks()
     achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "r02_stream_traffic.json")
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            if tj.get("csrc_sha") == _csrc_sha():
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), "profiles/r02_stream_traffic.json (ncu --set full of this build)"
-            else:
-                traffic_src = "profiles/r02_stream_traffic.json is from another build of the kernels: not reported"
-        except Exception:
-            pass
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "kernel": "dm_k_stream<false,false> (one launch per 64k-record message)",
                 "kernel_ms": kernel_ms, "kernel_ms_definition": "timed region / launches (consecutive launches overlap)",
                 "kernel_ms_isolated": (k_ms / k_n) if k_n else None,
@@ -623,12 +639,18 @@ def main():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step to DIR/*.npy")
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline legs")
     ap.add_argument("--no-extra", action="store_true", help="skip the config 3 / config 5 legs")
     args = ap.parse_args()
     if os.environ.get("DM_BENCH_WATCHDOG"):                    # a hung run says where: all threads' stacks every N seconds
         import faulthandler
         faulthandler.dump_traceback_later(float(os.environ["DM_BENCH_WATCHDOG"]), repeat=True, file=sys.stderr)
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs: the reference arm times a CPU restatement whose outputs are not kept; "
+                 "dump the GPU arm's outputs instead")
     if args.warmup < 3:
         args.warmup = 3
     if args.impl == "reference":

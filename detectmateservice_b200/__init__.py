@@ -1,4 +1,4 @@
-"""detectmateservice_b200 -- the DetectMate detector-stage hot path on B200 (sm_100a).
+"""detectmateservice_b200 -- the DetectMate detector-stage hot path on H100 (sm_90a).
 
 Scope (DESIGN.md): Engine._run_loop -> Service.process -> NewValueDetector of
 ait-detectmate/DetectMateService, rebuilt as CUDA kernels behind a C ABI

@@ -1,4 +1,4 @@
-"""Build and load libdmdetect.so (the sm_100a CUDA library behind include/dmdetect.h).
+"""Build and load libdmdetect.so (the sm_90a CUDA library behind include/dmdetect.h).
 
 There is no CPU fallback: if the library is missing or cannot be loaded this module
 raises, and every compute entry point of the library itself fails without a CUDA device
@@ -18,7 +18,7 @@ SO_PATH = os.environ.get("DM_LIB_PATH") or os.path.join(PKG_DIR, "libdmdetect.so
 HEADER = os.path.join(os.path.dirname(PKG_DIR), "include", "dmdetect.h")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 
@@ -48,7 +48,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """nvcc -gencode arch=compute_100a,code=sm_100a ... -> detectmateservice_b200/libdmdetect.so
+    """nvcc -gencode arch=compute_90a,code=sm_90a ... -> detectmateservice_b200/libdmdetect.so
     (in-tree, so the built library travels with the repo snapshot)."""
     if not force and not needs_build():
         return SO_PATH

@@ -126,7 +126,7 @@ class B200NewValueDetector(CoreComponent):
             method_type=cfg.get("method_type", "new_value_detector"),
             data_use_training=cfg.get("data_use_training"), auto_config=bool(cfg.get("auto_config", False))))
         if cfg.get("auto_config"):
-            raise ValueError("auto_config: true (a configure phase) is not supported by the B200 detector; "
+            raise ValueError("auto_config: true (a configure phase) is not supported by the CUDA detector; "
                              "list the monitored fields under global/events")
         self.detector_id = cfg.get("detector_id", "NewValueDetector" if name.startswith("B200") else name)
         self.method_type = cfg.get("method_type", "new_value_detector")
@@ -234,7 +234,7 @@ class B200NewValueDetector(CoreComponent):
     def reconfigure(self, config: Optional[Any]) -> bool:
         """Take a new detector configuration (what Service.reconfigure has just put into its config manager,
         /root/reference/src/service/core.py:299-345 -- the reference updates the manager and leaves the loaded
-        component alone; the B200 service subclass of service.py forwards it here).  Scalar parameters
+        component alone; the detector service subclass of service.py forwards it here).  Scalar parameters
         (data_use_training, output_format, start_id ...) apply in place and the known sets stay.  If the monitored
         fields, the log_format / templates or the device geometry change, the device handle is dropped and rebuilt
         on the next message: table keys are salted by the monitor's position, so the learnt state cannot be carried
@@ -374,10 +374,9 @@ class B200NewValueDetector(CoreComponent):
         merged = b"".join(o for o in outs if o)
         return merged or None
 
-    # Messages at least this large are cut into pieces that overlap copy and compute.  Measured on a B200 / PCIe 5 box
-    # (scripts/e2e_pieces.py): a piece costs ~150-280 us of latency (copy + kernel + two small copies back, each with a
-    # host synchronisation), so pieces below ~12 MiB LOSE against one call (16 MiB message: 0.42 ms in one call, 0.51 /
-    # 0.67 / 1.09 ms in 8 / 4 / 2 MiB pieces); from two 12 MiB pieces on the link stays busy (0.21 G records/s).
+    # Messages at least this large are cut into pieces that overlap copy and compute.  Every piece pays a fixed latency
+    # (copy + kernel + two small copies back, each with a host synchronisation), so small pieces lose against one call;
+    # scripts/e2e_pieces.py measures one call against 2 / 4 / 8 / 12 MiB pieces on the machine at hand.
     PIPE_MIN_BYTES = 24 << 20
     PIPE_PIECE_BYTES = 12 << 20
 

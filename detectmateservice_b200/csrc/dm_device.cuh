@@ -1,6 +1,6 @@
 // dm_device.cuh -- device-side data structures and helpers shared by the kernels.
 //
-// Compiles with nvcc for sm_100a (the product) and, with -DDM_EMU, with g++ against
+// Compiles with nvcc for sm_90a (the product) and, with -DDM_EMU, with g++ against
 // tests/emu/cuda_emu.h (CPU emulation used only by the test tier).
 #pragma once
 #ifdef DM_EMU

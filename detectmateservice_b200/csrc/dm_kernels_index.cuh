@@ -1,4 +1,4 @@
-// dm_kernels_index.cuh -- K_A, the row / record index of a message (sm_100a).
+// dm_kernels_index.cuh -- K_A, the row / record index of a message (sm_90a).
 //
 // dm_k_rowindex streams the message once (16-byte loads), counts the '\n' of every 512-byte row,
 // turns the counts into a global exclusive prefix (tiles of 64 rows, decoupled look-back with

@@ -1,4 +1,4 @@
-// dm_kernels_stream.cuh -- the "stream" variant of the fused tokenizer + detector (sm_100a), default.
+// dm_kernels_stream.cuh -- the "stream" variant of the fused tokenizer + detector (sm_90a), default.
 //
 // Replaces, per record: MatcherParser field extraction + NewValueDetector.train / .detect of the
 // un-vendored detectmatelibrary, which the reference drives one record at a time from

@@ -241,8 +241,8 @@ extern "C" int dm_create(int device, uint32_t n_keys, const uint8_t* keys_blob, 
     if (device < 0 || device >= n_dev) return dm_fail(DM_ERR_ARG, "device %d out of range (0..%d)", device, n_dev - 1);
     cudaDeviceProp prop;
     DM_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10)
-        return dm_fail(DM_ERR_NO_DEVICE, "device %d is sm_%d%d; libdmdetect is built for sm_100a only", device,
+    if (prop.major != 9 || prop.minor != 0)          // sm_90a code loads on compute capability 9.0 only
+        return dm_fail(DM_ERR_NO_DEVICE, "device %d is sm_%d%d; libdmdetect is built for sm_90a (H100) only", device,
                        prop.major, prop.minor);
     DM_CUDA(cudaSetDevice(device));
 

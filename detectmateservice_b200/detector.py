@@ -1,7 +1,7 @@
 """DeviceDetector -- thin ctypes wrapper of one libdmdetect handle (one GPU).
 
 Host code stays Python; all tokenizing, hashing, set membership and scoring run in the
-sm_100a kernels behind include/dmdetect.h.  PyTorch tensors are used only as device /
+sm_90a kernels behind include/dmdetect.h.  PyTorch tensors are used only as device /
 pinned-host buffer containers whose raw pointers are handed to the C ABI.
 """
 from __future__ import annotations
@@ -21,7 +21,7 @@ def _as_key_bytes(k: Union[str, bytes]) -> bytes:
 
 
 class DeviceDetector:
-    """NewValueDetector state (known-value table + running statistics) on one B200.
+    """NewValueDetector state (known-value table + running statistics) on one H100.
 
     keys: the monitored field names, in monitor order (field k <-> bit k of the masks).
     """

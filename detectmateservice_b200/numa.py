@@ -1,8 +1,7 @@
 """NUMA placement of pinned host buffers.
 
 A pinned buffer lives on the NUMA node of the thread that allocated it; when that is not the
-node the GPU's PCIe root hangs off, host -> device copies run at about half the link rate
-(measured on the B200 boxes: 16 MiB in ~560 us instead of ~311 us, `scripts/e2e_steps.py`).
+node the GPU's PCIe root hangs off, host -> device copies can run well below the link rate.
 `bound_to_gpu_node(device)` pins the calling thread to the GPU-local CPUs while the buffers
 are allocated (and first touched) and restores the affinity afterwards.  Pure host-side
 plumbing around the boundary; nothing here computes.

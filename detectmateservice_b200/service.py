@@ -1,4 +1,4 @@
-"""Engine loop mirror + service wrappers for the B200 detector.
+"""Engine loop mirror + service wrappers for the CUDA detector.
 
 Two ways to run the detector behind the reference's data channel:
 
@@ -151,7 +151,7 @@ class DetectorEngine:
 
 
 def b200_detector_service():
-    """Return a ``Service`` subclass bound to the B200 detector (needs the reference's
+    """Return a ``Service`` subclass bound to the CUDA detector (needs the reference's
     ``service`` package importable).  Usage::
 
         B200DetectorService = b200_detector_service()

@@ -5,7 +5,7 @@ features/config_loader.py:5, features/config_manager.py:9, features/component_re
 
 It is put on ``sys.path`` by ``detectmateservice_b200.compat.install_shims()`` only when the
 real library cannot be imported (it is not vendored in the reference and not installable
-offline), so that B200 components satisfy the loader's ``isinstance(..., CoreComponent)``
+offline), so that this project's components satisfy the loader's ``isinstance(..., CoreComponent)``
 check (component_loader.py:52-55) either way.  It contains no detector logic.
 """
 __shim__ = True

@@ -1,6 +1,6 @@
 """Multi-GPU plumbing: shard the record stream by line, one all-reduce per window.
 
-One process per GPU (torch.distributed, NCCL over NVLink on the B200 box).  Detection is a
+One process per GPU (torch.distributed, NCCL between the GPUs of one node).  Detection is a
 pure per-record lookup against read-only state, so the stream shards by record with no
 data-path collective; the only exchange is, once per window, ONE sum-all-reduce of a small
 uint64 buffer that carries

@@ -1,5 +1,5 @@
 /*
- * dmdetect.h -- C ABI of libdmdetect.so, the B200 (sm_100a) detector hot path.
+ * dmdetect.h -- C ABI of libdmdetect.so, the H100 (sm_90a) detector hot path.
  *
  * The reference has no FFI: its hot path is the Python call chain
  *   Engine._run_loop            /root/reference/src/service/features/engine.py:153-217
@@ -36,7 +36,7 @@ extern "C" {
 #define DM_OK 0
 #define DM_ERR_ARG (-1)       /* bad argument                                         */
 #define DM_ERR_CUDA (-2)      /* CUDA runtime / launch failure (see dm_last_error)    */
-#define DM_ERR_NO_DEVICE (-3) /* no usable sm_100 device: the product has no CPU path */
+#define DM_ERR_NO_DEVICE (-3) /* no usable sm_90 device: the product has no CPU path */
 #define DM_ERR_CAPACITY (-4)  /* batch larger than the handle was created for         */
 #define DM_ERR_TABLE_FULL (-5)/* known-set table over its load limit                  */
 #define DM_ERR_STATE (-6)     /* call not valid in the handle's current state         */

@@ -2,15 +2,15 @@
 the CPU oracle as its library component (BASELINE.md section 4).  MEASUREMENT INFRASTRUCTURE:
 only bench.py's CPU legs and tests/ use this module.
 
-Where the reference comes from: `baseline/_ref` (pip --target install of the unmodified
-reference, travels to the GPU box) or /root/reference/src when that exists; its two missing
+Where the reference comes from: `oracle/_ref` (a copy of the unmodified reference service made
+by `make -C oracle ref`, see `install()`); its two missing
 third-party imports (`pynng`, `detectmatelibrary.common.*`) are this repo's stand-ins
 (detectmateservice_b200/shims), real packages win when installed.
 
 Two figures, as the reference is deployed (one single-threaded service per process,
-/root/reference/src/service/features/engine.py:80-82):
+service/features/engine.py:80-82):
   inprocess_rate  one thread calling Service.process(record) in a loop (metrics + delegate,
-                  /root/reference/src/service/core.py:176-206);
+                  service/core.py:176-206);
   ipc_rate        P service processes, each with its engine loop on its own ipc PAIR0 socket
                   (engine.py:153-217), each fed by its own sender process with 1/P of the stream.
 """
@@ -25,20 +25,23 @@ import time
 from typing import List, Optional, Tuple
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_REF_CANDIDATES = [os.path.join(ROOT, "baseline", "_ref"), "/root/reference/src"]
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
+
+
+def install() -> None:
+    """Copy the reference service and its test-suite into oracle/_ref (oracle/Makefile, target `ref`)."""
+    import subprocess
+    subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-s", "ref"])
 
 
 def reference_path() -> Optional[str]:
-    for p in _REF_CANDIDATES:
-        if os.path.isdir(os.path.join(p, "service")):
-            return p
-    return None
+    return REF_DIR if os.path.isdir(os.path.join(REF_DIR, "service")) else None
 
 
 def _setup_imports() -> str:
     p = reference_path()
     if p is None:
-        raise RuntimeError("the reference service is neither in baseline/_ref nor in /root/reference/src")
+        raise RuntimeError("the reference service is not in oracle/_ref (make -C oracle ref)")
     if ROOT not in sys.path:
         sys.path.insert(0, ROOT)
     if p not in sys.path:

@@ -5,7 +5,7 @@ a MatcherParser stage (detectmatelibrary.parsers.template_matcher, configured at
 /root/reference/tests/library_integration/test_pipe_filereader_matcher_nvd.py:74-88
 with log_format ``type=<type> msg=audit(<Time>...): <Content>``) turns each line into a
 ParserSchema whose ``logFormatVariables`` map the detector's ``header_variables``
-read (docs/interfaces.md:138-204).  The B200 path fuses that step: one message is N
+read (docs/interfaces.md:138-204).  The CUDA path fuses that step: one message is N
 '\\n'-terminated raw lines and every ``key=value`` field of a line is addressable as
 a header variable.  The parser source is not in /root/reference, so this rule is
 *defined here* (SURVEY.md section 8c, R-tok) and the CUDA tokenizer must reproduce

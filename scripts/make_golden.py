@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Generate tests/golden/* from the reference checkout (run in the build container only;
-/root/reference does not exist on the GPU box, the committed fixtures travel instead).
+"""Generate tests/golden/* from a DetectMateService checkout: scripts/make_golden.py <checkout>.
+The tests read only the committed fixtures.
 
   audit_sample.log            a 420-record subset of the reference's sample audit log
                               (tests/library_integration/audit.log): the first 250 records,
@@ -13,18 +13,24 @@
   docs_golden.json            the documented NewValueDetector example
                               (docs/getting_started.md:423-435,510).
   audit_stats.json            probe statistics of the full audit.log (SURVEY 8c iv).
+  audit.log.xz                the full audit.log itself (test DATA, xz-compressed), against
+                              which test_oracle_golden.py checks audit_stats.json.
+  reference_schema_fields.json  name, number, type, label of every field of the wire schemas,
+                              decoded from the descriptor in container/fluentout/schemas_pb.rb:8.
   audit_templates.txt         the nine `<*>` templates of the reference's parser test data
                               (tests/library_integration/audit_templates.txt; test DATA, copied
                               verbatim as a fixture like audit_sample.log).
 """
 import collections
 import json
+import lzma
 import os
+import re
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else None
 OUT = os.path.join(ROOT, "tests", "golden")
 
 from oracle.nvd import NewValueDetectorOracle  # noqa: E402
@@ -35,11 +41,54 @@ KEYS = ["type", "exe", "terminal", "acct", "res"]
 N_TRAIN = 200
 
 
+def _ruby_unescape(s: str) -> bytes:
+    out = bytearray()
+    i = 0
+    simple = {"n": 10, "r": 13, "t": 9, '"': 34, "\\": 92, "e": 27, "a": 7, "b": 8, "f": 12, "v": 11, "0": 0, "#": 35}
+    while i < len(s):
+        c = s[i]
+        if c != "\\":
+            out += c.encode("latin-1")
+            i += 1
+            continue
+        n = s[i + 1]
+        if n == "x":
+            m = re.match(r"[0-9a-fA-F]{1,2}", s[i + 2:i + 4])
+            out.append(int(m.group(0), 16))
+            i += 2 + len(m.group(0))
+        elif n in "01234567":
+            m = re.match(r"[0-7]{1,3}", s[i + 1:i + 4])
+            out.append(int(m.group(0), 8))
+            i += 1 + len(m.group(0))
+        else:
+            out.append(simple[n])
+            i += 2
+    return bytes(out)
+
+
+def schema_fields() -> dict:
+    """Fields of the messages of the reference's wire-schema descriptor (and of their map entries)."""
+    from google.protobuf import descriptor_pb2
+    src = open(os.path.join(REF, "container/fluentout/schemas_pb.rb"), "r", encoding="latin-1").read()
+    lit = re.search(r'descriptor_data = "((?:[^"\\]|\\.)*)"', src, re.S).group(1)
+    ref = descriptor_pb2.FileDescriptorProto()
+    ref.ParseFromString(_ruby_unescape(lit))
+    return {"source": "container/fluentout/schemas_pb.rb:8 of DetectMateService (descriptor of schemas.proto)",
+            "messages": {m.name: {
+                "fields": sorted([f.name, f.number, f.type, f.label, f.proto3_optional] for f in m.field),
+                "nested": {n.name: {"map_entry": n.options.map_entry, "fields": [[x.name, x.number, x.type] for x in n.field]}
+                           for n in m.nested_type}} for m in ref.message_type}}
+
+
 def main() -> None:
+    if REF is None:
+        raise SystemExit("usage: scripts/make_golden.py <DetectMateService checkout>")
     os.makedirs(OUT, exist_ok=True)
     with open(os.path.join(REF, "tests/library_integration/audit_templates.txt"), "rb") as f:
         open(os.path.join(OUT, "audit_templates.txt"), "wb").write(f.read())
     raw = open(os.path.join(REF, "tests/library_integration/audit.log"), "rb").read()
+    open(os.path.join(OUT, "audit.log.xz"), "wb").write(lzma.compress(raw, preset=9 | lzma.PRESET_EXTREME))
+    json.dump(schema_fields(), open(os.path.join(OUT, "reference_schema_fields.json"), "w"), indent=1, sort_keys=True)
     lines = rtok.split_records(raw)
     counts = collections.Counter(l.split(b" ")[0][5:].decode() for l in lines)
     rare = {t for t, c in counts.items() if c <= 4}

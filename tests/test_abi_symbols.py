@@ -28,10 +28,10 @@ def test_header_symbols_all_exported():
     assert lib.dm_abi_version() == 4
 
 
-def test_sass_is_sm100a_only():
+def test_sass_is_sm90a_only():
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", _lib.SO_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out and "sm_80" not in out
+    assert "sm_90a" in out and "sm_100" not in out and "sm_80" not in out
 
 
 def test_host_side_table_key_matches_spec():

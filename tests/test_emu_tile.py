@@ -1,5 +1,5 @@
 """The key=value kernels' SOURCES (dm_kernels_stream.cuh, dm_kernels_lanes.cuh), compiled for the CPU emulator in
-tests/emu, against the oracle.  Runs in the CPU tier; the same cases run on the B200
+tests/emu, against the oracle.  Runs in the CPU tier; the same cases run on the H100
 through the C ABI in test_gpu_parity.py.  (Emulation is test infrastructure: one thread
 block on OS threads -- it checks logic, not memory-model or multi-CTA behaviour.)
 """

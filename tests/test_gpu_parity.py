@@ -1,4 +1,4 @@
-"""Parity of the CUDA path (through the C ABI) with the oracle.  Needs a B200.
+"""Parity of the CUDA path (through the C ABI) with the oracle.  Needs an H100.
 
 Bars: flags bit-exact; scores within 1e-5 (they are small integers, so in practice exact);
 unknown-field masks, anomaly lists and statistics exact; learnt key sets equal to the
