@@ -91,6 +91,8 @@ struct DmxShared {
     unsigned long long zero_bound[DMX_NPAR]; // [seq % NPAR]: records of detect message seq-NPAR: launch seq's CTAs zero-fill
                                              // that many output entries between them, its epilogue does the rest (if any)
     unsigned int slow_batches[DMX_NPAR];     // [seq % NPAR]: field-phase batches of launch seq that held a candidate
+    unsigned int error;                      // DM_DEVERR_* bits of every launch with error_acc set since the host last
+                                             // read and cleared them (dm_sync): a later header no longer hides them
 };
 
 struct DmxArgs {
@@ -123,6 +125,8 @@ struct DmxArgs {
     const unsigned long long* bound_ptr;     // message with training AND detection records: byte offset of the
                                              // first detection record (dm_k_bound), else NULL
     uint32_t keep_error;                     // the epilogue ORs into hdr->error instead of assigning it
+    unsigned int* error_acc;                 // the detect epilogue also ORs the header's final error bits into this word
+                                             // (&sh->error), or NULL
     unsigned long long* timeline;            // diagnostics (DM_STREAM_TIMELINE=1): per CTA {smid, t_start, t_rows_done, t_exit},
                                              // then 8 epilogue stamps (globaltimer ns); else NULL
     uint32_t keytab_bytes;                   // bytes of the key table that go to shared memory (multiple of 16)
@@ -1124,7 +1128,9 @@ __device__ __forceinline__ void dmx_epilogue(const DmxArgs& a, unsigned long lon
             unsigned int err = (n_lines > a.max_lines || n_lines > a.out_cap) ? DM_DEVERR_TOO_MANY_LINES : 0u;
             if (staged > a.alert_cap) err |= DM_DEVERR_ANOMALY_OVERFLOW;
             a.hdr->n_anomalies = 0; a.hdr->anomaly_list_count = 0;
-            a.hdr->error = a.keep_error ? (a.hdr->error | err) : err;
+            err = a.keep_error ? (a.hdr->error | err) : err;     // (keep_error: dm_k_bound cleared it, TRAIN inserts set bits)
+            a.hdr->error = err;
+            if (a.error_acc && err) atomicOr(a.error_acc, err);
             a.hdr->n_newlines = nl;
             a.hdr->n_lines = n_lines;
             const unsigned long long tr = a.n_train_lines < n_lines ? a.n_train_lines : n_lines;
@@ -1344,11 +1350,12 @@ static inline void dmx_scratch_destroy(DmxScratch* s) {
     *s = DmxScratch();
 }
 
-// Enqueue the kernels for one message.  Returns the number of kernels launched or < 0.
+// Enqueue the kernels for one message.  Returns the number of kernels launched or < 0.  accumulate_errors: the message's
+// error bits also go to the handle's error word (DmxShared::error), for callers whose header a later message overwrites.
 static inline int dmx_launch(DmxScratch* s, const uint8_t* d_buf, uint64_t nbytes, uint64_t n_train_lines, DmTable table,
                              uint8_t* d_flags, float* d_scores, uint64_t out_cap, dm_anomaly_t* d_anoms, uint32_t anomaly_cap,
                              DmBatchHeader* d_hdr, unsigned long long* d_stats, uint64_t max_lines, cudaStream_t st,
-                             bool allow_overlap, void (*mark)(void*, cudaStream_t, int), void* mark_ctx) {
+                             bool allow_overlap, bool accumulate_errors, void (*mark)(void*, cudaStream_t, int), void* mark_ctx) {
     const uint32_t n_rows = (uint32_t)((nbytes + DMX_ROW - 1) / DMX_ROW);
     const uint32_t b_rows = (uint32_t)((nbytes + DMB_ROW - 1) / DMB_ROW);
     if (n_rows == 0) return 0;
@@ -1359,6 +1366,7 @@ static inline int dmx_launch(DmxScratch* s, const uint8_t* d_buf, uint64_t nbyte
     a.flags = d_flags; a.scores = d_scores; a.out_cap = out_cap; a.anomalies = d_anoms; a.anomaly_cap = anomaly_cap;
     a.hdr = d_hdr; a.stats = d_stats; a.n_train_lines = n_train_lines; a.max_lines = max_lines;
     a.sh = s->d_shared; a.alert_cap = s->alert_cap; a.bound_ptr = nullptr; a.keep_error = 0; a.timeline = s->d_timeline; a.ring_smem = DMX_RING_SMEM;
+    a.error_acc = accumulate_errors ? &s->d_shared->error : nullptr;
     a.keytab_bytes = s->dyn_smem - (uint32_t)DMX_RING_SMEM;
     a.hint = s->h_hint;                                      // (unified addressing: the mapped host pointer is the device pointer)
     // chained re-check when, in the last message whose epilogue has run, at least every fourth row had a batch with a

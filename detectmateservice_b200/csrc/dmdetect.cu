@@ -72,6 +72,7 @@ struct dm_handle {
     float* d_scores = nullptr;
     DmBatchHeader* d_hdr = nullptr;
     DmBatchHeader* h_hdr = nullptr;      // pinned
+    unsigned int* h_err = nullptr;       // pinned: the stream kernel's error word (DmxShared::error) as dm_sync last read it
     dm_anomaly_t* d_anoms = nullptr;
     uint32_t anomaly_cap = 0;
     unsigned long long* d_stats = nullptr;         // DM_STATS_WORDS
@@ -186,6 +187,8 @@ static int dm_create_fill(dm_handle* h, int device, const cudaDeviceProp& prop, 
     DM_CUDA(cudaMemset(h->d_hdr, 0, sizeof(DmBatchHeader)));
     DM_CUDA(cudaHostAlloc(&h->h_hdr, sizeof(DmBatchHeader), cudaHostAllocDefault));
     memset(h->h_hdr, 0, sizeof(DmBatchHeader));
+    DM_CUDA(cudaHostAlloc(&h->h_err, sizeof(unsigned int), cudaHostAllocDefault));
+    *h->h_err = 0;
     h->anomaly_cap = (uint32_t)std::min<uint64_t>(h->max_lines, 1u << 20);
     DM_CUDA(cudaMalloc(&h->d_anoms, (uint64_t)h->anomaly_cap * sizeof(dm_anomaly_t)));
     DM_CUDA(cudaMalloc(&h->d_stats, 3 * DM_STATS_WORDS * sizeof(unsigned long long)));
@@ -306,7 +309,7 @@ extern "C" int dm_destroy(dm_handle* h) {
     dmx_scratch_destroy(&h->dmx);
     cudaFree(h->d_keys); cudaFree(h->d_in);
     cudaFree(h->d_line_start); cudaFree(h->d_flags); cudaFree(h->d_scores); cudaFree(h->d_hdr);
-    cudaFreeHost(h->h_hdr); cudaFree(h->d_anoms); cudaFree(h->d_stats); cudaFreeHost(h->h_stats);
+    cudaFreeHost(h->h_hdr); cudaFreeHost(h->h_err); cudaFree(h->d_anoms); cudaFree(h->d_stats); cudaFreeHost(h->h_stats);
     cudaFree(h->table.slots); cudaFree(h->table.novel); cudaFree(h->table.count);
     cudaFree(h->d_vals); cudaFree(h->d_masks); cudaFree(h->d_mons); cudaFree(h->d_fmt); cudaFree(h->d_norm);
     for (int k = 0; k < 2; ++k) {
@@ -340,6 +343,21 @@ static int dm_check_device_errors(dm_handle* h) {
     if (err & DM_DEVERR_TOO_MANY_LINES)
         return dm_fail(DM_ERR_CAPACITY, "batch holds more than max_lines=%llu records", (unsigned long long)h->max_lines);
     return DM_OK;
+}
+
+// The header only holds the last message's errors; the stream kernel ORs those of every message enqueued by
+// dm_process_lines into the handle's error word as well.  Enqueues on st the copy of that word to h_err and its
+// clearing: after st is synchronised, dm_header_with_errors folds it into h_hdr.
+static int dm_fetch_errors(dm_handle* h, cudaStream_t st) {
+    DM_CUDA(cudaMemcpyAsync(h->h_err, &h->dmx.d_shared->error, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemsetAsync(&h->dmx.d_shared->error, 0, sizeof(unsigned int), st));
+    return DM_OK;
+}
+
+static int dm_header_with_errors(dm_handle* h) {
+    h->h_hdr->error |= *h->h_err;
+    *h->h_err = 0;
+    return dm_check_device_errors(h);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -430,7 +448,7 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     } else {
         stream_kernel = true;
         const int rc = dmx_launch(&h->dmx, d_buf, nbytes, n_train_lines, h->table, d_flags, d_scores, out_cap, h->d_anoms,
-                                  h->anomaly_cap, h->d_hdr, h->d_stats, h->max_lines, st, h->dmx.overlap, dm_prof_mark_cb, h);
+                                  h->anomaly_cap, h->d_hdr, h->d_stats, h->max_lines, st, h->dmx.overlap, true, dm_prof_mark_cb, h);
         if (rc < 0) return dm_fail(DM_ERR_CUDA, "stream kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         h->launches += (uint64_t)rc;
     }
@@ -441,8 +459,10 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     if (!want_sync) return DM_OK;
 
     DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
+    int rc = dm_fetch_errors(h, st);
+    if (rc != DM_OK) return rc;
     DM_CUDA(cudaStreamSynchronize(st));
-    int rc = dm_check_device_errors(h);
+    rc = dm_header_with_errors(h);
     if (rc != DM_OK) return rc;
     const uint64_t n_lines = h->h_hdr->n_lines;
     if (n_lines_out) *n_lines_out = n_lines;
@@ -783,7 +803,7 @@ extern "C" int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t n
     DM_CUDA(cudaStreamWaitEvent(st, sl.ev_in, 0));
     if (nbytes == 0) DM_CUDA(cudaMemsetAsync(sl.d_hdr, 0, sizeof(DmBatchHeader), st));
     const int launched = dmx_launch(&h->dmx, sl.d_in, nbytes, n_train_lines, h->table, sl.d_flags, sl.d_scores, h->max_lines, sl.d_anoms,
-                                    h->anomaly_cap, sl.d_hdr, h->d_stats, h->max_lines, st, true, dm_prof_mark_cb, h);
+                                    h->anomaly_cap, sl.d_hdr, h->d_stats, h->max_lines, st, true, false, dm_prof_mark_cb, h);
     if (launched < 0) return dm_fail(DM_ERR_CUDA, "stream kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     h->launches += (uint64_t)launched;
     DM_CUDA(cudaEventRecord(sl.ev_comp, st));
@@ -848,8 +868,10 @@ extern "C" int dm_sync(dm_handle* h, uint64_t* n_lines_out, uint64_t* n_anomalie
     if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
     DM_CUDA(cudaSetDevice(h->device));
     DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, h->last_stream));
+    int rc = dm_fetch_errors(h, h->last_stream);
+    if (rc != DM_OK) return rc;
     DM_CUDA(cudaStreamSynchronize(h->last_stream));
-    int rc = dm_check_device_errors(h);
+    rc = dm_header_with_errors(h);
     if (rc != DM_OK) return rc;
     if (n_lines_out) *n_lines_out = h->h_hdr->n_lines;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;

@@ -94,8 +94,9 @@ int dm_destroy(dm_handle* h);
  *                      Either may be NULL (results then stay in the handle's own buffers).
  *   n_lines_out/n_anomalies_out : host pointers, may be NULL.  If both are NULL and no host
  *                      output was requested the call only ENQUEUES work on `stream` and
- *                      returns without synchronising (device-resident pipelines);
- *                      otherwise it returns after the results are complete.
+ *                      returns without synchronising (device-resident pipelines; its errors are reported by
+ *                      the next dm_sync or synchronous call); otherwise it returns after the results are
+ *                      complete.
  * By default a call is ordered behind everything enqueued on `stream` before it.  After
  * dm_set_overlap(h, 1) consecutive device-resident detection calls on one stream overlap
  * (programmatic dependent launch): a call may then start READING its `buf` and the known-set
@@ -217,7 +218,12 @@ int dm_collect(dm_handle* h, uint32_t slot, const uint8_t** flags_out, const flo
 /* Anomalous records of the batch last collected from `slot` (same format as dm_get_anomalies). */
 int dm_collect_anomalies(dm_handle* h, uint32_t slot, dm_anomaly_t* out, uint32_t cap, uint32_t* n_out);
 
-/* Wait for everything enqueued on the handle and report the last batch's counts. */
+/* Wait for everything enqueued on the handle and report the last batch's counts.  On the default key=value kernel
+ * the error reported is that of ANY dm_process_lines call since the last dm_sync or synchronous dm_process_lines (a
+ * message with more records than out_cap_lines or max_lines, a training message that filled the known-set table, an
+ * anomaly list that overflowed), not only of the last one: an enqueued message whose outputs are wrong or truncated
+ * is not hidden by a good message behind it.  Reporting them clears them.  (DM_KERNEL=lanes, log_format mode and
+ * combination monitors report the last call's errors only.) */
 int dm_sync(dm_handle* h, uint64_t* n_lines_out, uint64_t* n_anomalies_out);
 
 /* The anomalous records of the last batch, sorted by record index (at most cap; *n_out is

@@ -122,10 +122,17 @@ static int emu_stream_run(EmuHandle* h, bool chained, const uint8_t* msg, uint64
     uint8_t* buf = (uint8_t*)aligned_alloc(64, ((nbytes + 64 + 63) / 64) * 64 + 64);
     memcpy(buf, msg, nbytes);
     for (int i = 0; i < 64; ++i) buf[nbytes + i] = (i & 1) ? '\n' : '=';      // hostile slack
-    memset(&h->hdr, 0, sizeof(h->hdr));
+    // as dm_process_lines: the header is the previous call's until this call's epilogue rewrites it (its take-out of
+    // the previous call's alerts reads it), except for an empty message; errors are read as dm_sync reads them
     *n_lines = 0; *n_anoms = 0; *err = 0;
     const uint32_t n_rows = (uint32_t)((nbytes + DMX_ROW - 1) / DMX_ROW);
-    if (n_rows == 0) { free(buf); return 0; }
+    if (n_rows == 0) {
+        memset(&h->hdr, 0, sizeof(h->hdr));
+        *err = g_xs.sh.error;
+        g_xs.sh.error = 0;
+        free(buf);
+        return 0;
+    }
     for (unsigned b = 0; b < DMX_NPAR; ++b) {
         if (g_xs.row_cnt[b].size() < n_rows + 1) g_xs.row_cnt[b].assign(n_rows + 1, 0xBEEF);
         if (g_xs.alerts[b].size() < h->anoms.size()) g_xs.alerts[b].resize(h->anoms.size());
@@ -139,6 +146,7 @@ static int emu_stream_run(EmuHandle* h, bool chained, const uint8_t* msg, uint64
     a.hdr = &h->hdr; a.stats = h->stats; a.n_train_lines = n_train; a.max_lines = h->max_lines;
     a.sh = &g_xs.sh; a.alert_cap = (uint32_t)h->anoms.size(); a.bound_ptr = nullptr; a.keep_error = 0; a.timeline = nullptr; a.ring_smem = DMX_RING_SMEM;
     a.hint = &g_xs.hint;
+    a.error_acc = &g_xs.sh.error;
     a.keytab_bytes = (uint32_t)((DMX_KEYTAB_HOT(g_xs.tab.l1_slots) + 15) & ~(size_t)15);
     const unsigned long long warps_max = (unsigned long long)g_emu_stream_ctas * DMX_WARPS;
     const uint32_t rpw = (uint32_t)((n_rows + warps_max - 1) / warps_max);
@@ -169,7 +177,8 @@ static int emu_stream_run(EmuHandle* h, bool chained, const uint8_t* msg, uint64
     free(buf);
     *n_lines = h->hdr.n_lines;
     *n_anoms = h->hdr.n_anomalies;
-    *err = h->hdr.error;
+    *err = h->hdr.error | g_xs.sh.error;
+    g_xs.sh.error = 0;
     return 0;
 }
 

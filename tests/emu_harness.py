@@ -64,10 +64,16 @@ class EmuDetector:
             self.lib.emu_destroy(self.h)
             self.h = None
 
-    def process_lines(self, msg: bytes, n_train: int = 0):
-        cap = msg.count(b"\n") + 2
-        flags = np.full(cap, 7, dtype=np.uint8)
-        scores = np.full(cap, -1, dtype=np.float32)
+    def process_lines(self, msg: bytes, n_train: int = 0, out=None):
+        """out: (flags u8, scores f32) arrays owned by the caller, written in place (capacity = their length), as a
+        device-resident caller passes the same buffers to call after call; default: fresh ones pre-filled with 7 / -1."""
+        if out is None:
+            cap = msg.count(b"\n") + 2
+            flags = np.full(cap, 7, dtype=np.uint8)
+            scores = np.full(cap, -1, dtype=np.float32)
+        else:
+            flags, scores = out
+            cap = min(flags.size, scores.size)
         n_lines, n_anom, err = C.c_uint64(), C.c_uint64(), C.c_uint32()
         fn = {"lanes": self.lib.emu_process_lanes, "stream": self.lib.emu_process_stream,
               "chain": self.lib.emu_process_stream_chain}[self.variant]

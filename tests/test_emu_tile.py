@@ -12,6 +12,7 @@ import pytest
 import emu_harness
 from oracle import fingerprint
 from oracle.native import NativeOracle
+import util
 from util import FUZZ_KEYS, FUZZ_KEYS_FEW, fuzz_lines, lookalike_lines
 
 
@@ -216,4 +217,132 @@ def test_emu_everything_unknown():
     det = EmuDetector(keys)
     f, s = _check(det, o, msg, 0)
     assert f.all() and (s == 5).all()
+    det.close()
+
+
+def _emu_lib():
+    import ctypes as C
+    return C.CDLL(emu_harness.build())
+
+
+def test_emu_byte_position_sweep():
+    """'=' on every residue mod 32 and at the 1 KiB row edges, the first '=' at bytes 1-4, values ending before, at and
+    behind the 32-byte window and the 64 bytes behind a row, quoted spaces around the window's end, messages ending
+    inside a value for every nbytes % 16; about half of the values learnt.  Stream variants also with many short warp
+    segments (40 CTAs)."""
+    train, _ = util.sweep_training(0)
+    msgs = util.sweep_messages(0)
+    o = NativeOracle(util.SWEEP_KEYS)
+    det = EmuDetector(util.SWEEP_KEYS)
+    _check(det, o, train, train.count(b"\n"))
+    alerts = 0
+    for m in msgs:
+        f, _ = _check(det, o, m, 0)
+        alerts += int(f.sum())
+    assert alerts > len(msgs) // 2
+    if VARIANT != "lanes":
+        lib = _emu_lib()
+        lib.emu_stream_ctas(40)
+        try:
+            for m in msgs:
+                _check(det, o, m, 0)
+        finally:
+            lib.emu_stream_ctas(3)
+    det.close()
+
+
+def test_emu_keys32():
+    """One key of every length 1..32 (last four bytes shared along a chain, a suffix key, a byte >= 0x80): records
+    with all 32 fields and look-alikes; then nothing learnt: mask 0xFFFFFFFF and score 32."""
+    keys = util.KEYS32
+    assert sorted(len(k) for k in keys) == list(range(1, 33))
+    train, known = util.keys32_training(1)
+    o = NativeOracle(keys)
+    det = EmuDetector(keys)
+    _check(det, o, train, train.count(b"\n"))
+    f, _ = _check(det, o, util.keys32_lines(2, 60, known=known), 0)
+    assert 0 < f.sum() < f.size
+    det.close()
+    o2 = NativeOracle(keys)
+    det2 = EmuDetector(keys)
+    msg = util.keys32_lines(3, 12)
+    f, s = _check(det2, o2, msg, 0)
+    assert f.all() and (s == 32).all()
+    assert {a[1] for a in det2.anomalies()} == {0xFFFFFFFF}
+    st = det2.stats()
+    assert st["unknown_per_key"] == [12] * 32 and st["score_sum"] == 12 * 32
+    det2.close()
+
+
+def test_emu_keys32_three_byte_level1_table():
+    """32 distinct 3-byte keys: 96 level-1 patterns, the 512-slot table."""
+    _default_variant_only()
+    keys = util.KEYS32_3BYTE
+    train, known = util.keys32_training(4, keys=keys)
+    o = NativeOracle(keys)
+    det = EmuDetector(keys)
+    _check(det, o, train, train.count(b"\n"))
+    f, _ = _check(det, o, util.keys32_lines(5, 40, keys=keys, known=known), 0)
+    assert 0 < f.sum() < f.size
+    det.close()
+
+
+def test_emu_train_detect_split_sweep():
+    """Every split point of a ~3 KB message of 40 records (several 512-byte rows of dm_k_bound, no newline at the
+    end), each with a fresh detector."""
+    _default_variant_only()
+    keys = [b"type", b"res", b"acct"]
+    msg = util.split_message(6)
+    n = msg.count(b"\n") + 1
+    assert len(msg) > 4 * 512 and n == 40
+    for n_train in range(n + 3):
+        o = NativeOracle(keys)
+        det = EmuDetector(keys)
+        _check(det, o, msg, n_train)
+        st = det.stats()
+        assert st["train_lines"] == min(n_train, n) and st["lines"] == n
+        assert st["unknown_per_key"] == [o.unknown_count(i) for i in range(len(keys))]
+        assert st["known_keys"] == sum(o.known_count(i) for i in range(len(keys)))
+        det.close()
+
+
+def test_emu_train_detect_split_per_group():
+    """More than 256 rows of 512 bytes: dm_k_bound finds the split through its per-thread groups of rows; n_train at
+    records that hold a group edge."""
+    _default_variant_only()
+    keys = [b"type", b"res", b"acct"]
+    msg = util.split_message(7, n_records=2000, mean_len=90)
+    rows = (len(msg) + 511) // 512
+    assert rows > 256
+    per = (rows + 255) // 256
+    arr = np.frombuffer(msg, dtype=np.uint8)
+    nl = np.nonzero(arr == 10)[0]
+    for grp in (1, 2, 100, 255):
+        edge = grp * per * 512
+        rec = int(np.searchsorted(nl, edge))                           # the record holding byte `edge`
+        for n_train in (rec - 1, rec, rec + 1):
+            o = NativeOracle(keys)
+            det = EmuDetector(keys)
+            _check(det, o, msg, n_train)
+            det.close()
+
+
+def test_emu_shared_output_buffer():
+    """One caller-owned output buffer, pre-filled with 7 / -1 once, through messages whose record counts grow and shrink
+    across the 4-set rotation: the zero-fill bound left by the call four back, the epilogue's rest and its take-out of
+    the previous call's alerts."""
+    keys = [b"type", b"res", b"acct"]
+    msgs = [util.split_message(s, n_records=n) for s, n in
+            [(10, 300), (11, 5), (12, 1), (13, 250), (14, 40), (15, 400), (16, 2), (17, 350), (18, 30), (19, 120)]]
+    msgs.insert(3, b"")
+    msgs.insert(6, b"\n")
+    o = NativeOracle(keys)
+    det = EmuDetector(keys)
+    flags = np.full(512, 7, dtype=np.uint8)
+    scores = np.full(512, -1, dtype=np.float32)
+    _check(det, o, msgs[0], 200)
+    for m in msgs[1:]:
+        f, s = det.process_lines(m, 0, out=(flags, scores))
+        wf, ws, _ = o.process(m, 0)
+        assert f.tolist() == wf.tolist() and s.tolist() == ws.tolist()
     det.close()

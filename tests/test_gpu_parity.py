@@ -376,3 +376,120 @@ def test_pipelined_submit_collect(monkeypatch, kernel="stream"):
         det.collect(0)
         st = det.stats()
         assert st["lines"] == sum(w[0].size for w in want) + 5000 and st["train_lines"] == 3000
+
+
+def _check_device(det, oracle, msg, n_train, stream):
+    """_check through the device-resident path: the message in a device buffer with exactly 16 bytes of hostile
+    slack, outputs in device buffers pre-filled with 7 / -1."""
+    import torch
+    host = np.concatenate([np.frombuffer(msg, dtype=np.uint8), np.frombuffer(b"=\n" * 8, dtype=np.uint8)])
+    x = torch.from_numpy(host).cuda()
+    cap = msg.count(b"\n") + 1
+    flags = torch.full((cap,), 7, dtype=torch.uint8, device="cuda")
+    scores = torch.full((cap,), -1.0, dtype=torch.float32, device="cuda")
+    torch.cuda.synchronize()
+    det.enqueue_device(x.data_ptr(), len(msg), n_train, flags.data_ptr(), scores.data_ptr(), cap, stream.cuda_stream)
+    n, _ = det.sync()
+    of, os_, om = oracle.process(msg, n_train, want_masks=True)
+    assert n == of.size
+    f, s = flags.cpu().numpy()[:n], scores.cpu().numpy()[:n]
+    bad = np.nonzero(f != of)[0]
+    assert bad.size == 0, f"flags differ at records {bad[:10]} (gpu {f[bad[:10]]}, oracle {of[bad[:10]]})"
+    assert (s == os_).all()
+    an = det.anomalies()
+    idx = np.nonzero(of)[0]
+    assert [a[0] for a in an] == idx.tolist() and [a[1] for a in an] == om[idx].tolist()
+    return f, s
+
+
+def test_byte_position_sweep(variant):
+    """tests/util.sweep_messages: '=' on every residue mod 32 and at the 1 KiB row edges, first '=' at bytes 1-4,
+    value lengths around the 32-byte window and the 64 bytes behind a row, quoted spaces at the window's end, messages
+    ending inside a value for every nbytes % 16.  Host path and device buffers with exactly 16 bytes of slack."""
+    import torch
+    import util
+    train, _ = util.sweep_training(0)
+    msgs = util.sweep_messages(0)
+    stream = torch.cuda.Stream()
+    for device in (False, True):
+        o = NativeOracle(util.SWEEP_KEYS)
+        with _det(util.SWEEP_KEYS) as det:
+            _check(det, o, train, train.count(b"\n"))
+            for m in msgs:
+                if device:
+                    _check_device(det, o, m, 0, stream)
+                else:
+                    _check(det, o, m, 0)
+
+
+def test_keys32(variant):
+    """One key of every length 1..32 (shared last four bytes, a suffix key, a byte >= 0x80) with look-alikes; then
+    nothing learnt: every record alerts on all 32 fields."""
+    import util
+    keys = util.KEYS32
+    train, known = util.keys32_training(1)
+    o = NativeOracle(keys)
+    with _det(keys) as det:
+        _check(det, o, train, train.count(b"\n"))
+        f, _ = _check(det, o, util.keys32_lines(2, 2000, known=known), 0)
+        assert 0 < f.sum() < f.size
+        st = det.stats()
+        assert st["unknown_per_key"] == [o.unknown_count(i) for i in range(32)]
+    o2 = NativeOracle(keys)
+    with _det(keys) as det:
+        f, s = _check(det, o2, util.keys32_lines(3, 500), 0)
+        assert f.all() and (s == 32).all()
+        assert {a[1] for a in det.anomalies()} == {0xFFFFFFFF}
+        st = det.stats()
+        assert st["unknown_per_key"] == [500] * 32 and st["score_sum"] == 500 * 32
+
+
+def test_keys32_three_byte_level1_table_full_message(variant):
+    """32 distinct 3-byte keys (96 level-1 patterns: the 512-slot table, 4 KiB more shared memory per CTA) on a full
+    64k x 256 B message."""
+    import util
+    keys = util.KEYS32_3BYTE
+    train, known = util.keys32_training(4, keys=keys)
+    o = NativeOracle(keys)
+    with _det(keys) as det:
+        _check(det, o, train, train.count(b"\n"))
+        rng = np.random.Generator(np.random.PCG64(8))
+        recs = []
+        for i in range(65536):
+            js = rng.choice(32, 12, replace=False)
+            toks = [keys[j] + b"=" + (known[j][int(rng.integers(0, len(known[j])))] if rng.random() < 0.99 else b"n%d" % i)
+                    for j in js]
+            rec = b" ".join(toks)
+            recs.append(rec + b" " + b"p" * max(0, 255 - len(rec) - 1) if len(rec) < 254 else rec[:255])
+        msg = b"\n".join(recs) + b"\n"
+        assert msg.count(b"\n") == 65536
+        f, _ = _check(det, o, msg, 0)
+        assert 0 < f.sum() < f.size
+
+
+def test_train_detect_split_sweep(variant):
+    """Every split point 0 .. n+2 of a ~3 KB message of 40 records crossing several 512-byte rows of dm_k_bound (tail
+    record without a newline), each with a fresh detector; then a message of more than 256 such rows (dm_k_bound's
+    per-group path) split at records that hold a group edge."""
+    import util
+    keys = [b"type", b"res", b"acct"]
+    msg = util.split_message(6)
+    n = msg.count(b"\n") + 1
+    for n_train in range(n + 3):
+        o = NativeOracle(keys)
+        with _det(keys, max_batch_bytes=1 << 20, table_log2_slots=12) as det:
+            _check(det, o, msg, n_train)
+            st = det.stats()
+            assert st["train_lines"] == min(n_train, n) and st["lines"] == n
+            assert st["unknown_per_key"] == [o.unknown_count(i) for i in range(len(keys))]
+            assert st["known_keys"] == sum(o.known_count(i) for i in range(len(keys)))
+    big = util.split_message(7, n_records=2000, mean_len=90)
+    rows = (len(big) + 511) // 512
+    per = (rows + 255) // 256
+    nl = np.nonzero(np.frombuffer(big, dtype=np.uint8) == 10)[0]
+    for grp in (1, 2, 100, 255):
+        rec = int(np.searchsorted(nl, grp * per * 512))
+        for n_train in (rec - 1, rec, rec + 1):
+            o = NativeOracle(keys)
+            with _det(keys, max_batch_bytes=1 << 20, table_log2_slots=12) as det:
+                _check(det, o, big, n_train)
