@@ -319,18 +319,26 @@ class B200NewValueDetector(CoreComponent):
         return {self.monitors[i].alert_key: _alerts.alert_text(by_field.get(i, b""))
                 for i in range(len(self.monitors)) if mask >> i & 1}
 
+    def _bad_records(self) -> int:
+        """The device's count of malformed records (0 for a device stand-in that keeps no statistics)."""
+        stats = getattr(self.det, "stats", None)
+        return int(stats()["bad_records"]) if stats else 0
+
     def _process_record_batch(self, data: bytes) -> Optional[bytes]:
         """A message holding many length-delimited ParserSchema records: field walk, monitor
         matching, hashing and scoring happen on the device; the host only decodes the (rare)
         anomalous records to word their alerts."""
         remaining = max(0, self.data_use_training - self.n_seen)
+        bad0 = self._bad_records()
         try:
             flags, scores, masks = self.det.process_records(data, n_train_records=remaining)
         except Exception as e:
             self._count_dropped_training(e, remaining, lambda: len(wire.split_delimited(data)))
             raise
         n = int(flags.size)
-        self.n_seen += n
+        # malformed records take no training slot (as on the per-record path, where they raise before counting)
+        self.last_n_malformed = self._bad_records() - bad0
+        self.n_seen += n - self.last_n_malformed
         if self.output_format == "compact":
             return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
         if self.det.last_n_anomalies == 0:
@@ -592,6 +600,8 @@ class B200NewValueComboDetector(B200NewValueDetector):
 
     def _process_record(self, data: bytes) -> Optional[bytes]:
         out = self._process_record_batch(wire.frame_delimited([data]))     # the device walks the record
+        if self.last_n_malformed:
+            raise wire.WireError("malformed ParserSchema record")          # as B200NewValueDetector's per-record path
         if out is None or self.output_format == "compact":
             return out
         return wire.split_delimited(out)[0]                                 # one record in, one bare alert out

@@ -8,6 +8,11 @@
 //                 10 logFormatVariables map<string,string> (entry: 1 key, 2 value)
 //   every other field is skipped by wire type.
 //
+// Well-formed (DESIGN.md section 5.3): a record is walked exactly as protobuf's runtime parses ParserSchema -- tags of
+// at most 5 bytes below 2^32 and not field 0, every fixed32/fixed64/LEN payload inside the record, strict UTF-8 in the
+// string fields and in map keys and values -- except that a group (wire types 3/4) makes the record malformed.  A
+// malformed record has flag, score and mask 0, is counted in stats word 7 (bad_records) and never trains.
+//
 // Monitor semantics (R-spec 3, DESIGN.md): a global monitor applies to every record, an
 // event monitor only when record.EventID matches; header monitors read
 // logFormatVariables[KEY] (last entry wins, as in protobuf maps), variable monitors read
@@ -70,9 +75,135 @@ __device__ __forceinline__ bool dm_pb_varint(const uint8_t* __restrict__ buf, ui
     return false;
 }
 
-__global__ void __launch_bounds__(128) dm_k_records(DmRecordsArgs a, int phase) {
-    // phase 0: training records insert; phase 1: the others are scored (separate launches so
-    // that detection sees every insert)
+// A tag as protobuf's runtime reads it: at most 5 bytes, below 2^32, field number not 0.
+__device__ __forceinline__ bool dm_pb_tag(const uint8_t* __restrict__ buf, uint32_t& pos, uint32_t end, uint32_t& field, uint32_t& wt) {
+    uint64_t v = 0;
+    for (uint32_t shift = 0; shift < 35; shift += 7) {
+        if (pos >= end) return false;
+        const uint32_t b = buf[pos++];
+        v |= (uint64_t)(b & 0x7Fu) << shift;
+        if (!(b & 0x80u)) {
+            field = (uint32_t)(v >> 3);
+            wt = (uint32_t)v & 7u;
+            return (v >> 32) == 0 && field != 0;
+        }
+    }
+    return false;
+}
+
+// Skips the payload of a field protobuf does not know (or knows under another wire type).  Groups (wire types 3/4)
+// are refused: proto3 cannot declare them, so no ParserSchema producer emits them -- the one deliberate divergence
+// from protobuf's runtime, which skips a group as an unknown field.
+__device__ __forceinline__ bool dm_pb_skip(const uint8_t* __restrict__ buf, uint32_t& pos, uint32_t end, uint32_t wt) {
+    uint64_t v;
+    switch (wt) {
+        case 0: return dm_pb_varint(buf, pos, end, v);
+        case 1: if (end - pos < 8u) return false; pos += 8; return true;
+        case 5: if (end - pos < 4u) return false; pos += 4; return true;
+        case 2:
+            if (!dm_pb_varint(buf, pos, end, v) || v > (uint64_t)(end - pos)) return false;
+            pos += (uint32_t)v;
+            return true;
+        default: return false;
+    }
+}
+
+// Strict UTF-8 (what protobuf's runtime checks in every proto3 string): no overlong forms, no surrogates, nothing
+// above U+10FFFF, no sequence cut short.
+__device__ __forceinline__ bool dm_utf8_ok(const uint8_t* __restrict__ s, uint32_t n) {
+    uint32_t i = 0;
+    while (i < n) {
+        const uint32_t c = s[i];
+        if (c < 0x80u) { ++i; continue; }
+        uint32_t need, lo = 0x80u, hi = 0xBFu;
+        if (c >= 0xC2u && c <= 0xDFu) need = 1;
+        else if (c >= 0xE0u && c <= 0xEFu) { need = 2; if (c == 0xE0u) lo = 0xA0u; else if (c == 0xEDu) hi = 0x9Fu; }
+        else if (c >= 0xF0u && c <= 0xF4u) { need = 3; if (c == 0xF0u) lo = 0x90u; else if (c == 0xF4u) hi = 0x8Fu; }
+        else return false;
+        if (n - i <= need) return false;
+        const uint32_t c1 = s[i + 1];
+        if (c1 < lo || c1 > hi) return false;
+        for (uint32_t j = 2; j <= need; ++j)
+            if ((s[i + j] & 0xC0u) != 0x80u) return false;
+        i += need + 1;
+    }
+    return true;
+}
+
+// The string fields of ParserSchema (1 2 3 5 6 7 8 9; 10 is the map, its keys and values are strings too).
+DM_HD bool dm_pb_string_field(uint32_t f) { return f <= 9u && ((0x3EEu >> f) & 1u); }
+
+// Walks one ParserSchema record [pos, end).  Returns false exactly where protobuf's runtime refuses the record (and for
+// a group anywhere in it); else vp/vl/present hold the monitored values and eid/has_eid the EventID, as protobuf reads
+// them: the last EventID wins, variables[i] is the i-th field 6, logFormatVariables[key] the last entry with that key.
+// A map entry holding anything but LEN fields 1 and 2 is dropped, as protobuf's runtime drops it (its key and value are
+// still checked for UTF-8); an absent key or value reads as "".
+__device__ __forceinline__ bool dm_pb_walk_record(const uint8_t* __restrict__ buf, uint32_t pos, const uint32_t end,
+                                                  const DmMonitors& sm, uint32_t* vp, uint32_t* vl, uint32_t& present,
+                                                  int32_t& eid, bool& has_eid) {
+    uint32_t var_idx = 0;
+    while (pos < end) {
+        uint32_t field, wt;
+        if (!dm_pb_tag(buf, pos, end, field, wt)) return false;
+        if (wt == 0 && field == 4) {
+            uint64_t v;
+            if (!dm_pb_varint(buf, pos, end, v)) return false;
+            eid = (int32_t)(uint32_t)v;
+            has_eid = true;
+            continue;
+        }
+        if (wt != 2) {
+            if (!dm_pb_skip(buf, pos, end, wt)) return false;
+            continue;
+        }
+        uint64_t len64;
+        if (!dm_pb_varint(buf, pos, end, len64) || len64 > (uint64_t)(end - pos)) return false;
+        const uint32_t len = (uint32_t)len64;
+        if (dm_pb_string_field(field) && !dm_utf8_ok(buf + pos, len)) return false;
+        if (field == 6) {
+            for (uint32_t k = 0; k < sm.n; ++k)
+                if (sm.m[k].source == 1 && sm.m[k].var_index == var_idx) { vp[k] = pos; vl[k] = len; present |= 1u << k; }
+            ++var_idx;
+        } else if (field == 10) {
+            uint32_t p = pos, kp = pos, kl = 0, xp = pos, xl = 0;      // key, value (absent = empty)
+            const uint32_t e = pos + len;
+            bool foreign = false;
+            while (p < e) {
+                uint32_t f2, w2;
+                if (!dm_pb_tag(buf, p, e, f2, w2)) return false;
+                if (w2 != 2 || (f2 != 1 && f2 != 2)) {
+                    if (!dm_pb_skip(buf, p, e, w2)) return false;
+                    foreign = true;
+                    continue;
+                }
+                uint64_t l2;
+                if (!dm_pb_varint(buf, p, e, l2) || l2 > (uint64_t)(e - p)) return false;
+                if (!dm_utf8_ok(buf + p, (uint32_t)l2)) return false;
+                if (f2 == 1) { kp = p; kl = (uint32_t)l2; }
+                else { xp = p; xl = (uint32_t)l2; }
+                p += (uint32_t)l2;
+            }
+            if (!foreign) {
+                for (uint32_t k = 0; k < sm.n; ++k) {
+                    if (sm.m[k].source != 0 || sm.m[k].key_len != kl) continue;
+                    bool eq = true;
+                    for (uint32_t i = 0; i < kl; ++i)
+                        if (buf[kp + i] != sm.m[k].key[i]) { eq = false; break; }
+                    if (eq) { vp[k] = xp; vl[k] = xl; present |= 1u << k; }
+                }
+            }
+        }
+        pos += len;
+    }
+    return true;
+}
+
+// phase 2: mark each record well-formed (flags[r] = 1) or not, for dm_k_records_bound;
+// phase 0: the records before the split insert (training); phase 1: the others are scored (separate launches so that
+// detection sees every insert).  Every record writes its outputs in phase 0 or 1.
+// bound: {first scored record, records trained} from dm_k_records_bound, which puts the split just past the
+// n_train_records-th WELL-FORMED record; NULL splits at record n_train_records itself (the same when it is 0).
+__global__ void __launch_bounds__(128) dm_k_records(DmRecordsArgs a, int phase, const uint32_t* bound_in = nullptr) {
     __shared__ DmMonitors sm;
     {
         const uint32_t* src = reinterpret_cast<const uint32_t*>(a.mons);
@@ -81,63 +212,22 @@ __global__ void __launch_bounds__(128) dm_k_records(DmRecordsArgs a, int phase) 
     }
     __syncthreads();
     const uint8_t* __restrict__ buf = a.buf;
+    const uint32_t bound = bound_in ? bound_in[0] : a.n_train_records;
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.n_records; r += gridDim.x * blockDim.x) {
-        const bool train = r < a.n_train_records;
-        if (train != (phase == 0)) continue;
+        const bool train = r < bound;
+        if (phase != 2 && train != (phase == 0)) continue;
         uint32_t vp[DM_MAX_KEYS], vl[DM_MAX_KEYS];
         uint32_t present = 0;
-        uint32_t pos = a.rec_off[r];
-        const uint32_t end = pos + a.rec_len[r];
         int32_t eid = 0;
         bool has_eid = false;
-        uint32_t var_idx = 0;
-        bool ok = true;
-        while (ok && pos < end) {
-            uint64_t tag;
-            if (!dm_pb_varint(buf, pos, end, tag)) { ok = false; break; }
-            const uint32_t field = (uint32_t)(tag >> 3), wt = (uint32_t)(tag & 7u);
-            if (wt == 0) {
-                uint64_t v;
-                if (!dm_pb_varint(buf, pos, end, v)) { ok = false; break; }
-                if (field == 4) { eid = (int32_t)(uint32_t)v; has_eid = true; }
-            } else if (wt == 2) {
-                uint64_t len64;
-                if (!dm_pb_varint(buf, pos, end, len64) || len64 > (uint64_t)(end - pos)) { ok = false; break; }
-                const uint32_t len = (uint32_t)len64;
-                if (field == 6) {
-                    for (uint32_t k = 0; k < sm.n; ++k)
-                        if (sm.m[k].source == 1 && sm.m[k].var_index == var_idx) { vp[k] = pos; vl[k] = len; present |= 1u << k; }
-                    ++var_idx;
-                } else if (field == 10) {
-                    uint32_t p = pos, kp = 0, kl = 0, xp = pos, xl = 0;      // key, value (absent = empty)
-                    const uint32_t e = pos + len;
-                    bool eok = true;
-                    while (p < e) {
-                        uint64_t t2, l2;
-                        if (!dm_pb_varint(buf, p, e, t2) || (t2 & 7u) != 2u || !dm_pb_varint(buf, p, e, l2) || l2 > (uint64_t)(e - p)) { eok = false; break; }
-                        if ((t2 >> 3) == 1) { kp = p; kl = (uint32_t)l2; }
-                        else if ((t2 >> 3) == 2) { xp = p; xl = (uint32_t)l2; }
-                        p += (uint32_t)l2;
-                    }
-                    if (!eok) { ok = false; break; }
-                    for (uint32_t k = 0; k < sm.n; ++k) {
-                        if (sm.m[k].source != 0 || sm.m[k].key_len != kl) continue;
-                        bool eq = true;
-                        for (uint32_t i = 0; i < kl; ++i)
-                            if (buf[kp + i] != sm.m[k].key[i]) { eq = false; break; }
-                        if (eq) { vp[k] = xp; vl[k] = xl; present |= 1u << k; }
-                    }
-                }
-                pos += len;
-            } else if (wt == 1) {
-                pos += 8;
-            } else if (wt == 5) {
-                pos += 4;
-            } else {
-                ok = false;
-            }
+        const uint32_t pos = a.rec_off[r];
+        const bool ok = dm_pb_walk_record(buf, pos, pos + a.rec_len[r], sm, vp, vl, present, eid, has_eid);
+        if (phase == 2) { a.flags[r] = ok ? 1 : 0; continue; }
+        if (!ok) {                                                // malformed record: counted, never trained or scored
+            a.flags[r] = 0; a.scores[r] = 0.0f; a.masks[r] = 0;
+            atomicAdd(a.stats + 7, 1ull);
+            continue;
         }
-        if (!ok) { atomicAdd(a.stats + 7, 1ull); continue; }     // malformed record: counted, not scored
         uint32_t unknown = 0, have = 0;
         uint64_t fpv[DM_MAX_KEYS];
         for (uint32_t k = 0; k < sm.n; ++k) {
@@ -180,5 +270,34 @@ __global__ void __launch_bounds__(128) dm_k_records(DmRecordsArgs a, int phase) 
         } else {
             a.flags[r] = 0; a.scores[r] = 0.0f; a.masks[r] = 0;
         }
+    }
+}
+
+// One CTA, after phase 2: bound[0] = the index just past the n_train-th well-formed record (n_records if the batch
+// holds fewer), bound[1] = the well-formed records before it, i.e. the records trained.  Training counts well-formed
+// records only, as the per-record path does (a malformed record raises before it takes a training slot).
+__global__ void __launch_bounds__(256) dm_k_records_bound(const uint8_t* __restrict__ ok, uint32_t n_records,
+                                                          uint32_t n_train, uint32_t* bound) {
+    __shared__ uint32_t s_sum[256];
+    const uint32_t tid = threadIdx.x;
+    const uint32_t per = (n_records + 255) / 256;
+    const uint32_t lo = tid * per < n_records ? tid * per : n_records;
+    const uint32_t hi = lo + per < n_records ? lo + per : n_records;
+    uint32_t s = 0;
+    for (uint32_t r = lo; r < hi; ++r) s += ok[r];
+    s_sum[tid] = s;
+    __syncthreads();
+    if (tid == 0) {
+        uint32_t run = 0, t = 0;
+        while (t < 256 && run + s_sum[t] < n_train) { run += s_sum[t]; ++t; }
+        uint32_t b = n_records;
+        if (t < 256) {
+            uint32_t r = t * per;
+            for (;; ++r)
+                if (ok[r] && ++run == n_train) break;
+            b = r + 1;
+        }
+        bound[0] = b;
+        bound[1] = run;
     }
 }

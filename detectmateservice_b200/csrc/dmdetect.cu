@@ -702,7 +702,7 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
-    if (2ull * n_records > 3ull * h->vals_cap) {
+    if (2ull * n_records + 2 > 3ull * h->vals_cap + 1) {
         if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
         h->vals_cap = std::max<uint64_t>(2ull * n_records, 4096);
         DM_CUDA(cudaMalloc(&h->d_vals, (3 * h->vals_cap + 1) * sizeof(uint32_t)));
@@ -710,12 +710,11 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     if (!h->d_masks) DM_CUDA(cudaMalloc(&h->d_masks, (h->max_lines + 4) * sizeof(uint32_t)));
     uint32_t* d_off = h->d_vals;
     uint32_t* d_len = h->d_vals + n_records;
+    uint32_t* d_bound = h->d_vals + 2ull * n_records;             // {first scored record, records trained}
+    uint32_t bound[2] = {0, 0};
     DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
     if (n_records) {
-        // (the kernel skips malformed records without touching their outputs: they read as "no alert")
-        DM_CUDA(cudaMemsetAsync(h->d_flags, 0, n_records, st));
-        DM_CUDA(cudaMemsetAsync(h->d_scores, 0, (uint64_t)n_records * 4, st));
-        DM_CUDA(cudaMemsetAsync(h->d_masks, 0, (uint64_t)n_records * 4, st));
+        // (every record writes its flag, score and mask in the train or the detect launch, malformed ones included)
         DM_CUDA(cudaMemcpyAsync(h->d_in, buf, nbytes, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync(d_off, off.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync(d_len, len.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
@@ -724,10 +723,17 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
         a.mons = h->d_mons; a.table = h->table; a.flags = h->d_flags; a.scores = h->d_scores; a.masks = h->d_masks;
         a.hdr = h->d_hdr; a.stats = h->d_stats;
         const int grid = (int)std::min<uint32_t>((n_records + 127) / 128, (uint32_t)h->sm_count * 16);
-        if (n_train_records > 0) { dm_k_records<<<grid, 128, 0, st>>>(a, 0); h->launches++; }
+        if (n_train_records > 0) {
+            // training takes the first n_train_records WELL-FORMED records: mark them (flags as scratch), find the
+            // bound, then insert.  Batches after training skip both extra launches.
+            dm_k_records<<<grid, 128, 0, st>>>(a, 2);
+            dm_k_records_bound<<<1, 256, 0, st>>>(h->d_flags, n_records, n_train_records, d_bound);
+            dm_k_records<<<grid, 128, 0, st>>>(a, 0, d_bound);
+            h->launches += 3;
+        }
         if (n_train_records < n_records) {
             dm_prof_mark(h, st, 0);
-            dm_k_records<<<grid, 128, 0, st>>>(a, 1);
+            dm_k_records<<<grid, 128, 0, st>>>(a, 1, n_train_records > 0 ? d_bound : nullptr);
             dm_prof_mark(h, st, 1);
             h->launches++;
         }
@@ -737,12 +743,14 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     if (flags_out && n_records) DM_CUDA(cudaMemcpyAsync(flags_out, h->d_flags, n_records, cudaMemcpyDeviceToHost, st));
     if (scores_out && n_records) DM_CUDA(cudaMemcpyAsync(scores_out, h->d_scores, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
     if (masks_out && n_records) DM_CUDA(cudaMemcpyAsync(masks_out, h->d_masks, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
+    if (n_records && n_train_records > 0) DM_CUDA(cudaMemcpyAsync(bound, d_bound, sizeof(bound), cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
     {
-        const unsigned long long tr = std::min<uint32_t>(n_train_records, n_records);
+        // train_lines: the records trained; detect_lines: the records from the bound on (malformed ones included)
+        const unsigned long long tr = bound[1], first_scored = n_train_records > 0 ? bound[0] : 0;
         unsigned long long cur[6];
         DM_CUDA(cudaMemcpy(cur, h->d_stats, sizeof(cur), cudaMemcpyDeviceToHost));
-        unsigned long long upd[3] = {cur[0] + n_records, cur[1] + tr, cur[2] + (n_records - tr)};
+        unsigned long long upd[3] = {cur[0] + n_records, cur[1] + tr, cur[2] + (n_records - first_scored)};
         const unsigned long long nb = cur[5] + nbytes;
         DM_CUDA(cudaMemcpy(h->d_stats, upd, sizeof(upd), cudaMemcpyHostToDevice));
         DM_CUDA(cudaMemcpy(h->d_stats + 5, &nb, sizeof(nb), cudaMemcpyHostToDevice));

@@ -80,15 +80,54 @@ _PARSER_VARINT = {4, 11, 12}
 _PARSER_NAMES = {1: "__version__", 2: "parserType", 3: "parserID", 5: "template", 7: "parsedLogID", 8: "logID", 9: "log"}
 
 
+def _read_tag(buf: bytes, pos: int) -> Tuple[int, int, int]:
+    """(field, wire type, pos) as protobuf's runtime reads a tag: at most 5 bytes, below 2^32, field not 0."""
+    start = pos
+    tag, pos = _read_varint(buf, pos)
+    if pos - start > 5 or tag >> 32:
+        raise WireError("tag out of range")
+    if tag >> 3 == 0:
+        raise WireError("field number 0")
+    return tag >> 3, tag & 7, pos
+
+
+def _skip_field(buf: bytes, pos: int, end: int, wt: int) -> int:
+    """Position after the payload of a field that is not read.  Groups (wire types 3/4) raise: proto3 cannot declare
+    them, so a ParserSchema holding one is refused (protobuf's runtime would skip it)."""
+    if wt == 0:
+        _, pos = _read_varint(buf, pos)
+    elif wt == 1:
+        pos += 8
+    elif wt == 5:
+        pos += 4
+    elif wt == 2:
+        ln, pos = _read_varint(buf, pos)
+        pos += ln
+    else:
+        raise WireError(f"unexpected wire type {wt}")
+    if pos > end:
+        raise WireError("field runs past the end")
+    return pos
+
+
+def _utf8(b: bytes) -> str:
+    try:
+        return b.decode("utf-8")
+    except UnicodeDecodeError as e:
+        raise WireError(f"string field is not valid UTF-8: {e}") from None
+
+
 def decode_parser_schema(buf: bytes, strict: bool = True) -> Dict:
     """ParserSchema bytes -> dict with str values (EventID None when absent).
-    strict: unknown fields / wrong wire types raise WireError (used to tell a record from
-    raw log lines); otherwise unknown fields are skipped like protobuf does."""
+    Accepts and reads exactly what protobuf's runtime does (DESIGN.md section 5.3), except that a group raises:
+    invalid UTF-8 in a string field, map key or value, field 0, a tag of 2^32 or more, or a payload running past the
+    end raise WireError; a map entry holding anything but LEN fields 1 and 2 is dropped.
+    strict: unknown fields / wrong wire types, at the top level or in a map entry, raise WireError too (used to tell a
+    record from raw log lines); otherwise they are skipped like protobuf does."""
     rec: Dict = {"EventID": None, "variables": [], "logFormatVariables": {}, "logID": ""}
     pos, n = 0, len(buf)
     while pos < n:
-        tag, pos = _read_varint(buf, pos)
-        field, wt = tag >> 3, tag & 7
+        field, wt, pos = _read_tag(buf, pos)
         if wt == 2:
             ln, pos = _read_varint(buf, pos)
             end = pos + ln
@@ -96,25 +135,31 @@ def decode_parser_schema(buf: bytes, strict: bool = True) -> Dict:
                 raise WireError("length-delimited field runs past the end")
             if field == 10:
                 k = v = ""
+                foreign = False
                 p = pos
                 while p < end:
-                    t, p = _read_varint(buf, p)
-                    if t & 7 != 2:
-                        raise WireError("bad map entry")
+                    f2, w2, p = _read_tag(buf, p)
+                    if w2 != 2 or f2 not in (1, 2):
+                        if strict:
+                            raise WireError("bad map entry")
+                        p = _skip_field(buf, p, end, w2)
+                        foreign = True
+                        continue
                     l2, p = _read_varint(buf, p)
                     if p + l2 > end:
                         raise WireError("map entry runs past its end")
-                    s = buf[p:p + l2].decode("utf-8", "replace")
-                    if t >> 3 == 1:
+                    s = _utf8(buf[p:p + l2])
+                    if f2 == 1:
                         k = s
-                    elif t >> 3 == 2:
+                    else:
                         v = s
                     p += l2
-                rec["logFormatVariables"][k] = v
+                if not foreign:
+                    rec["logFormatVariables"][k] = v
             elif field == 6:
-                rec["variables"].append(buf[pos:end].decode("utf-8", "replace"))
+                rec["variables"].append(_utf8(buf[pos:end]))
             elif field in _PARSER_NAMES:
-                rec[_PARSER_NAMES[field]] = buf[pos:end].decode("utf-8", "replace")
+                rec[_PARSER_NAMES[field]] = _utf8(buf[pos:end])
             elif strict:
                 raise WireError(f"unexpected length-delimited field {field}")
             pos = end
@@ -128,14 +173,10 @@ def decode_parser_schema(buf: bytes, strict: bool = True) -> Dict:
                 rec["parsedTimestamp"] = _int32(v)
             elif strict:
                 raise WireError(f"unexpected varint field {field}")
-        elif wt == 5 and not strict:
-            pos += 4
-        elif wt == 1 and not strict:
-            pos += 8
-        else:
+        elif strict:
             raise WireError(f"unexpected wire type {wt} for field {field}")
-        if pos > n:
-            raise WireError("truncated message")
+        else:
+            pos = _skip_field(buf, pos, n, wt)
     return rec
 
 

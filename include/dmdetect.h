@@ -54,8 +54,9 @@ typedef struct {
     uint64_t score_sum;      /* sum of scores (scores are small integers)             */
     uint64_t bytes;          /* input bytes consumed                                  */
     uint64_t known_keys;     /* entries in the known-set table                        */
-    uint64_t bad_records;    /* records that could not be parsed (malformed protobuf,
-                                log_format mismatch): counted, never scored           */
+    uint64_t bad_records;    /* records that could not be parsed (malformed ParserSchema,
+                                see dm_process_records; log_format mismatch): counted,
+                                never trained or scored                               */
     uint64_t unknown_per_key[DM_MAX_KEYS]; /* alerts per monitored field             */
 } dm_stats_t;
 
@@ -132,9 +133,20 @@ int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blob_bytes, co
  * single bare record is the reference's native case and goes through dm_process_values).
  * The host only walks the length prefixes; the protobuf field walk, the monitor matching
  * (dm_set_monitors), dm_fp64, the table probe and the scoring run in one kernel, one thread
- * per record.  Records [0, n_train_records) are training data.  Host output buffers of
- * out_cap entries (any may be NULL).  Synchronous.  Replaces per-record
- * ParserSchema.deserialize + NewValueDetector.train/detect behind core.py:201-203. */
+ * per record.  Host output buffers of out_cap entries (any may be NULL).  Synchronous.
+ * Replaces per-record ParserSchema.deserialize + NewValueDetector.train/detect behind
+ * core.py:201-203.
+ * A record is well-formed if and only if protobuf's runtime parses it as ParserSchema
+ * (strict UTF-8 in every string field and map key / value, tags below 2^32 and not field 0,
+ * every payload inside the record), with one deliberate exception: a record holding a group
+ * (wire types 3/4) is malformed, where protobuf skips it (proto3 cannot declare groups).  A
+ * well-formed record yields the values protobuf yields; a map entry holding any field but
+ * LEN fields 1 and 2 is dropped, as protobuf drops it.  A malformed record gets flag, score
+ * and mask 0, is counted in dm_stats_t.bad_records and is never trained on.
+ * Training: the first n_train_records WELL-FORMED records train (malformed records take no
+ * training slot); every record from just past the n_train_records-th well-formed one is
+ * scored.  dm_stats_t.train_lines grows by the records trained; the bad_records delta of a
+ * call is the number of its malformed records. */
 typedef struct {
     int32_t event_id;     /* records with this EventID only ...                          */
     uint32_t has_event;   /* ... if non-zero; 0 = global scope (every record)            */

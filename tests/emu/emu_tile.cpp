@@ -238,10 +238,18 @@ extern "C" int emu_process_records(EmuHandle* h, const DmMonitor* mons, uint32_t
     DmRecordsArgs a;
     a.buf = msg; a.rec_off = off.data(); a.rec_len = len.data(); a.n_records = n; a.n_train_records = n_train;
     a.mons = &hm; a.table = h->table; a.flags = flags; a.scores = scores; a.masks = masks; a.hdr = &h->hdr; a.stats = h->stats;
+    uint32_t bound[2] = {0, 0};
     if (n) {
-        if (n_train > 0) emu_launch(128, [&] { dm_k_records(a, 0); });
-        if (n_train < n) emu_launch(128, [&] { dm_k_records(a, 1); });
+        if (n_train > 0) {
+            emu_launch(128, [&] { dm_k_records(a, 2); });
+            emu_launch(256, [&] { dm_k_records_bound(flags, n, n_train, bound); });
+            emu_launch(128, [&] { dm_k_records(a, 0, bound); });
+        }
+        if (n_train < n) emu_launch(128, [&] { dm_k_records(a, 1, n_train > 0 ? bound : nullptr); });
     }
+    h->stats[0] += n;
+    h->stats[1] += bound[1];
+    h->stats[2] += n - (n_train > 0 ? bound[0] : 0);
     *n_records = n;
     *n_anoms = h->hdr.n_anomalies;
     return 0;

@@ -92,7 +92,7 @@ class EmuDetector:
         w = (C.c_uint64 * 40)()
         self.lib.emu_get_stats(self.h, w)
         return {"lines": w[0], "train_lines": w[1], "detect_lines": w[2], "anomalies": w[3], "score_sum": w[4],
-                "bytes": w[5], "known_keys": w[6], "unknown_per_key": [w[8 + i] for i in range(len(self.keys))]}
+                "bytes": w[5], "known_keys": w[6], "bad_records": w[7], "unknown_per_key": [w[8 + i] for i in range(len(self.keys))]}
 
     def export_known(self):
         out = (C.c_uint64 * (1 << 16))()
