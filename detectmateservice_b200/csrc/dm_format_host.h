@@ -82,7 +82,8 @@ struct FmtBuilder {
             ++lits_here;
             f.chain_endcap[c] = 0;
         }
-        if (lits_here > DM_FMT_MAX_CHAIN_LITS) { err = "more than 32 captures in one log_format / template"; return false; }
+        const uint32_t caps_here = f.chain_endcap[c] ? lits_here : lits_here - 1;
+        if (caps_here > DM_FMT_MAX_CAPTURES) { err = "more than 32 captures in one log_format / template"; return false; }
         f.n_chains = c + 1;
         f.chain_first[c + 1] = (uint16_t)n_lits;
         return true;
@@ -127,7 +128,7 @@ inline bool dm_format_build(const char* log_format, const char* content_name, ui
             const std::string key((const char*)hm.m[k].key, hm.m[k].key_len);
             for (size_t i = 0; i < b.header_names.size(); ++i)
                 if (b.header_names[i] == key) b.f.mon_index[k] = (uint8_t)i;
-        } else if (hm.m[k].var_index < DM_FMT_MAX_CHAIN_LITS) {
+        } else if (hm.m[k].var_index < DM_FMT_MAX_CAPTURES) {
             b.f.mon_index[k] = (uint8_t)hm.m[k].var_index;
         }
     }

@@ -1,6 +1,6 @@
 // dm_kernels_format.cuh -- the MatcherParser step fused in front of the detector
 // (SURVEY.md section 8a8 / 8f-3): `log_format` header extraction and `<*>` template matching on
-// the device, one warp per record, feeding the same known-set table.
+// the device, one thread per record, feeding the same known-set table.
 //
 // What it replaces: detectmatelibrary.parsers.template_matcher.MatcherParser (un-vendored;
 // configured at /root/reference/tests/library_integration/test_pipe_filereader_matcher_nvd.py:74-88
@@ -24,7 +24,8 @@
 
 #define DM_FMT_MAX_CHAINS 64          // log_format + 63 templates
 #define DM_FMT_MAX_LITS 512           // literals over all chains
-#define DM_FMT_MAX_CHAIN_LITS 32      // literals (and captures) per chain: one capture per lane
+#define DM_FMT_MAX_CAPTURES 32        // captures per chain: capture i is bit i of chain_need (a chain has one more literal
+                                      // than captures when it ends with a literal)
 #define DM_FMT_POOL_WORDS 1024        // literal text over all chains, each literal padded to 4-byte words
 #define DM_FMT_MAX_LIT_LEN 255
 #define DM_FMT_NONE 0xFFu

@@ -14,8 +14,12 @@ from __future__ import annotations
 from typing import Dict, List, Optional, Sequence, Tuple
 
 _NAME_CHARS = frozenset(b"ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz0123456789_")
+# the device's limits (csrc/dm_kernels_format.cuh); LogFormat applies them all
 MAX_TEMPLATES = 63
-MAX_CAPTURES = 32
+MAX_CAPTURES = 32                    # per chain, whether it ends with a capture or with a literal
+MAX_LITERAL_BYTES = 255              # per literal; template literals after R-norm
+MAX_LITERALS = 512                   # over the log_format and all templates
+POOL_BYTES = 4096                    # literal text over the log_format and all templates, each literal padded to 4-byte words
 
 # R-norm (DESIGN.md): MatcherParser's params.remove_spaces / remove_punctuation / lowercase.  The same
 # bits are passed to dm_set_format_ex; the device drops / folds the same bytes (DmFormat.norm_drop).
@@ -73,7 +77,34 @@ class Chain:
         return caps
 
 
-def _parse(text: bytes, named: bool) -> Chain:
+class _LiteralBudget:
+    """The device's limits on literals over the log_format and all templates, checked literal by literal in the order
+    dm_format_build adds them, with its reasons (csrc/dm_format_host.h)."""
+
+    def __init__(self) -> None:
+        self.n_lits = 0
+        self.pool_words = 0
+
+    def add(self, lit: bytes) -> None:
+        if self.n_lits >= MAX_LITERALS:
+            raise ValueError("too many literals over the log_format and the templates")
+        if len(lit) > MAX_LITERAL_BYTES:
+            raise ValueError("a literal between two captures is longer than 255 bytes")
+        words = (len(lit) + 3) // 4
+        if self.pool_words + words > POOL_BYTES // 4:
+            raise ValueError("the literal text of log_format + templates exceeds 4096 bytes")
+        self.pool_words += words
+        self.n_lits += 1
+
+
+def _parse(text: bytes, named: bool, flags: int = 0, budget: Optional[_LiteralBudget] = None) -> Chain:
+    """One chain, checked as the device checks it.  Templates (named == False) are normalised literal by literal
+    (R-norm: every literal is normalised, the wildcards stay)."""
+    if budget is None:
+        budget = _LiteralBudget()
+    if b"\0" in text:
+        raise ValueError("a NUL byte (the device's configuration strings end at the first one)")
+    norm = (lambda s: s) if named else (lambda s: normalise(s, flags))
     lits: List[bytes] = []
     names: List[str] = []
     lit = bytearray()
@@ -97,30 +128,24 @@ def _parse(text: bytes, named: bool) -> Chain:
             last_cap = False
             continue
         if last_cap:
-            raise ValueError("two captures with nothing between them in %r" % text.decode("utf-8", "replace"))
-        lits.append(bytes(lit))
+            raise ValueError("two captures with nothing between them")
+        front = norm(bytes(lit))
+        if lits and front == b"":
+            raise ValueError("normalisation leaves nothing between two wildcards")
+        budget.add(front)                                          # the literal in front of this capture (L0 may be empty)
+        lits.append(front)
         lit = bytearray()
         names.append(name)
         last_cap = True
         i = end
-    if not last_cap:
-        lits.append(bytes(lit))
-    if len(lits) > MAX_CAPTURES:
-        raise ValueError("more than %d captures in %r" % (MAX_CAPTURES, text.decode("utf-8", "replace")))
-    return Chain(lits, last_cap, names)
-
-
-def _normalised(ch: Chain, flags: int, source: bytes) -> Chain:
-    """R-norm on a template: every literal is normalised, the wildcards stay."""
-    if not flags:
-        return ch
-    lits = [normalise(l, flags) for l in ch.literals]
-    inner = lits[1:] if ch.ends_with_capture else lits[1:-1]
-    if any(l == b"" for l in inner):
-        raise ValueError("normalisation leaves nothing between two wildcards of %r" % source.decode("utf-8", "replace"))
-    if not ch.ends_with_capture and len(lits) > 1 and lits[-1] == b"":
-        return Chain(lits[:-1], True, ch.names)                  # `... <*>'` -> the last wildcard runs to the end
-    return Chain(lits, ch.ends_with_capture, ch.names)
+    final = norm(bytes(lit))
+    ends = last_cap or (not named and flags != 0 and bool(lits) and final == b"")   # `... <*>'` normalised: runs to the end
+    if not ends:
+        budget.add(final)                                          # the final literal (or the whole text)
+        lits.append(final)
+    if (len(lits) if ends else len(lits) - 1) > MAX_CAPTURES:
+        raise ValueError("more than %d captures in one log_format / template" % MAX_CAPTURES)
+    return Chain(lits, ends, names)
 
 
 def _b(x) -> bytes:
@@ -128,19 +153,34 @@ def _b(x) -> bytes:
 
 
 class LogFormat:
+    """Raises ValueError on every configuration the device rejects, in dm_format_build's order and with its reasons,
+    so that a bad configuration fails where the component is constructed rather than at its first message."""
+
     def __init__(self, log_format, templates: Sequence = (), content_name: str = "Content", flags: int = 0) -> None:
         self.source = _b(log_format).decode("utf-8")
         self.template_sources = [_b(t) for t in templates]
         self.flags = int(flags)
-        self.header = _parse(_b(log_format), named=True)
-        if len(set(self.header.names)) != len(self.header.names):
-            raise ValueError("log_format: a capture name appears twice")
-        self.templates = [_normalised(_parse(_b(t), named=False), self.flags, _b(t)) for t in templates]
-        if len(self.templates) > MAX_TEMPLATES:
-            raise ValueError(f"{len(self.templates)} templates, the device holds {MAX_TEMPLATES}")
         self.content_name = content_name
-        if self.templates and content_name not in self.header.names:
+        if b"\0" in _b(content_name):
+            raise ValueError("content_name: a NUL byte (the device's configuration strings end at the first one)")
+        budget = _LiteralBudget()
+        try:
+            self.header = _parse(_b(log_format), named=True, budget=budget)
+        except ValueError as e:
+            raise ValueError("log_format: %s" % e) from None
+        for i, n in enumerate(self.header.names):
+            if n in self.header.names[:i]:
+                raise ValueError("log_format: capture <%s> appears twice" % n)
+        if self.template_sources and content_name not in self.header.names:
             raise ValueError(f"templates given but log_format has no <{content_name}> capture")
+        self.templates = []
+        for t, src in enumerate(self.template_sources):
+            try:
+                if t >= MAX_TEMPLATES:
+                    raise ValueError("too many templates (at most %d)" % MAX_TEMPLATES)
+                self.templates.append(_parse(src, named=False, flags=self.flags, budget=budget))
+            except ValueError as e:
+                raise ValueError("template %d: %s" % (t, e)) from None
 
     def parse(self, line: bytes) -> Optional[Tuple[int, List[bytes], Dict[str, bytes]]]:
         """(EventID, variables, header variables) of one record, None if log_format does not match."""

@@ -183,9 +183,12 @@ int dm_set_combos(dm_handle* h, uint32_t n_combos, const uint32_t* member_off, c
  *                (0-based, -1 = no match) and variables[i] = its i-th wildcard.
  * The monitors of dm_set_monitors are bound to it: header monitors by capture name, variable
  * monitors by wildcard index, event scope by EventID.  After this call dm_process_lines
- * tokenises with the log_format instead of key=value fields (one warp per record); records
+ * tokenises with the log_format instead of key=value fields (one thread per record); records
  * the log_format does not match are counted (dm_stats_t.bad_records) and never alert.
- * log_format = NULL switches back.  At most 63 templates, 32 captures per chain. */
+ * log_format = NULL switches back.  Limits (DM_ERR_ARG): at most 63 templates and 32 captures
+ * per chain; every literal at most 255 bytes (template literals after R-norm); at most 512
+ * literals and 4096 bytes of literal text over the log_format and all templates, each literal
+ * counted rounded up to whole 4-byte words.  The strings end at their first NUL byte. */
 int dm_set_format(dm_handle* h, const char* log_format, const char* content_name, uint32_t n_templates,
                   const char* const* templates);
 /* dm_set_format + MatcherParser's params.remove_spaces / remove_punctuation / lowercase
