@@ -453,11 +453,7 @@ class B200NewValueDetector(CoreComponent):
             rec = _alerts.record_at(data, offset)
             if self.logformat is not None:
                 _eid, variables, lfv = self.logformat.parse(rec) or (-1, [], {})
-                alerts = {}
-                for i, m in enumerate(self.monitors):
-                    if mask >> i & 1:
-                        v = lfv.get(m.pos, b"") if m.source == "header" else (variables[m.pos] if m.pos < len(variables) else b"")
-                        alerts[m.alert_key] = _alerts.alert_text(v)
+                alerts = self._format_alerts(variables, lfv, mask)
                 out.append(self._detector_schema(str(base + line_idx), float(scores[line_idx]), alerts, lfv.get("Time")))
                 continue
             alerts = self._line_alerts(rec, mask, raw_keys)
@@ -478,6 +474,16 @@ class B200NewValueDetector(CoreComponent):
                 self.n_seen += int(count())
             except Exception:
                 self.n_seen += remaining
+
+    @staticmethod
+    def _format_value(m: Monitor, variables: List[bytes], lfv: Dict[str, bytes]) -> bytes:
+        """Value of monitor m in a record LogFormat.parse split (variables are slices of the normalised Content)."""
+        return lfv.get(m.pos, b"") if m.source == "header" else (variables[m.pos] if m.pos < len(variables) else b"")
+
+    def _format_alerts(self, variables: List[bytes], lfv: Dict[str, bytes], mask: int) -> Dict[str, str]:
+        """alertsObtain of one anomalous record in log_format mode from the device's unknown-field mask."""
+        return {m.alert_key: _alerts.alert_text(self._format_value(m, variables, lfv))
+                for i, m in enumerate(self.monitors) if mask >> i & 1}
 
     def _line_alerts(self, rec: bytes, mask: int, raw_keys: List[bytes]) -> Dict[str, str]:
         """alertsObtain of one anomalous raw record from the device's unknown-field mask."""
@@ -556,23 +562,43 @@ def parse_combos(cfg: dict) -> Tuple[List[Monitor], List[List[int]]]:
     return mons, combos
 
 
+def check_format_combos(cfg: dict, lf) -> None:
+    """With a log_format, a combination one of whose members no record can ever have is dead configuration (one
+    missing member silences the whole tuple): a header variable that names no capture of the log_format, or a
+    template variable when no templates are configured.  Raises ValueError naming the instance."""
+    captures = set(lf.header.names)
+    scopes = [("global", cfg.get("global"))] + [("events.%s" % eid, sc) for eid, sc in (cfg.get("events") or {}).items()]
+    for where, scope in scopes:
+        for inst_name, inst in (scope or {}).items():
+            inst = inst or {}
+            for hv in inst.get("header_variables") or []:
+                if str(hv["pos"]) not in captures:
+                    raise ValueError(f"combination {where}.{inst_name}: header variable {str(hv['pos'])!r} is not a capture "
+                                     f"of the log_format, so the combination can never be complete")
+            if inst.get("variables") and not lf.templates:
+                raise ValueError(f"combination {where}.{inst_name}: template variables but no templates are configured, "
+                                 f"so the combination can never be complete")
+
+
 class B200NewValueComboDetector(B200NewValueDetector):
     """NewValueComboDetector on the device (SURVEY.md section 8f-4; semantics R-combo in DESIGN.md /
     oracle/nvcd.py): tuples of field values instead of single values.  The member
     fingerprints are folded in order into one 64-bit key and learnt / probed in the same
-    table (`dm_set_combos`).  Input: ParserSchema (one per message or a delimited batch), or raw
-    key=value records for combinations of global header variables."""
+    table (`dm_set_combos`).  Input: ParserSchema (one per message or a delimited batch), raw
+    key=value records for combinations of global header variables, or raw log lines split by
+    ``params.log_format`` / ``templates`` / ``path_templates`` (and the R-norm switches), where a
+    combination may mix header captures and the variables of its event's template.  A tuple
+    has the same key in all three, so known sets carry over (export_state / import_state)."""
 
     def __init__(self, name: str = "B200NewValueComboDetector", config: Optional[Any] = None) -> None:
         raw_cfg = config.model_dump() if hasattr(config, "model_dump") else config
         cfg = select_component_config(raw_cfg, name, fallback="NewValueComboDetector")
         cfg.setdefault("method_type", "new_value_combo_detector")
         cfg.setdefault("detector_id", "NewValueComboDetector" if name.startswith("B200") else name)
-        if cfg.get("log_format"):
-            raise ValueError("combination monitors are not evaluated in log_format mode; feed key=value records "
-                             "or ParserSchema messages")
         super().__init__(name=name, config={"detectors": {name: cfg}})
         self.monitors, self.combos = parse_combos(cfg)
+        if self.logformat is not None:
+            check_format_combos(cfg, self.logformat)
 
     @property
     def det(self):
@@ -585,18 +611,23 @@ class B200NewValueComboDetector(B200NewValueDetector):
     def _description(self) -> str:
         return f"{self.detector_id} detects value combinations not encountered in training as anomalies."
 
+    def _combo_alert(self, members: List[int], values: List[bytes]) -> Tuple[str, str]:
+        """("<scope> - (<label>, ...)", "Unknown value combination: ('v1', ...)") of one combination."""
+        m0 = self.monitors[members[0]]
+        scope = "Global" if m0.event_id is None else f"EventID {m0.event_id}"
+        key = "%s - (%s)" % (scope, ", ".join(self.monitors[i].label for i in members))
+        return key, "Unknown value combination: (%s)" % ", ".join("'%s'" % v.decode("utf-8", "replace") for v in values)
+
     def _record_alerts(self, rec: Dict, mask: int) -> Dict[str, str]:
         by_field = dict(self._record_values(rec))
         n = len(self.monitors)
-        out = {}
-        for c, members in enumerate(self.combos):
-            if mask >> (n + c) & 1:
-                m0 = self.monitors[members[0]]
-                scope = "Global" if m0.event_id is None else f"EventID {m0.event_id}"
-                key = "%s - (%s)" % (scope, ", ".join(self.monitors[i].label for i in members))
-                out[key] = "Unknown value combination: (%s)" % ", ".join(
-                    "'%s'" % by_field.get(i, b"").decode("utf-8", "replace") for i in members)
-        return out
+        return dict(self._combo_alert(members, [by_field.get(i, b"") for i in members])
+                    for c, members in enumerate(self.combos) if mask >> (n + c) & 1)
+
+    def _format_alerts(self, variables: List[bytes], lfv: Dict[str, bytes], mask: int) -> Dict[str, str]:
+        n = len(self.monitors)
+        return dict(self._combo_alert(members, [self._format_value(self.monitors[i], variables, lfv) for i in members])
+                    for c, members in enumerate(self.combos) if mask >> (n + c) & 1)
 
     def _process_record(self, data: bytes) -> Optional[bytes]:
         out = self._process_record_batch(wire.frame_delimited([data]))     # the device walks the record
@@ -626,11 +657,8 @@ class B200NewValueComboDetector(B200NewValueDetector):
         for c, members in enumerate(self.combos):
             if mask >> (n + c) & 1:
                 vals = _alerts.record_fields(rec, [raw_keys[i] for i in members])
-                m0 = self.monitors[members[0]]
-                scope = "Global" if m0.event_id is None else f"EventID {m0.event_id}"
-                key = "%s - (%s)" % (scope, ", ".join(self.monitors[i].label for i in members))
-                out[key] = "Unknown value combination: (%s)" % ", ".join(
-                    "'%s'" % vals.get(raw_keys[i], b"").decode("utf-8", "replace") for i in members)
+                key, text = self._combo_alert(members, [vals.get(raw_keys[i], b"") for i in members])
+                out[key] = text
         return out
 
 

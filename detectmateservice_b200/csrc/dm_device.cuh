@@ -199,7 +199,7 @@ struct DmDetectArgs {
     unsigned long long* stats;
     uint64_t line_lo, line_hi;        // records [line_lo, min(line_hi, n_lines)) are processed
     uint64_t nbytes;                  // message size
-    const void* combos;               // lanes kernel with combinations: const DmMonitors* (else NULL)
+    const void* combos;               // lanes / format kernel with combinations: const DmMonitors* (else NULL)
 };
 
 // ---------------------------------------------------------------------------------------

@@ -4,8 +4,8 @@
 //
 // What it replaces: detectmatelibrary.parsers.template_matcher.MatcherParser (un-vendored;
 // configured at /root/reference/tests/library_integration/test_pipe_filereader_matcher_nvd.py:74-88
-// and docs/getting_started.md:395-415) followed by NewValueDetector behind
-// /root/reference/src/service/core.py:201-203.  Rules: DESIGN.md R-fmt / R-match.
+// and docs/getting_started.md:395-415) followed by NewValueDetector or NewValueComboDetector behind
+// /root/reference/src/service/core.py:201-203.  Rules: DESIGN.md R-fmt / R-match / R-norm / R-combo.
 //
 //   chain     L0 C0 L1 C1 ... L(n-1) [C(n-1)]     literals L, captures C
 //   match     L0 anchored at the start; every later literal at its EARLIEST occurrence at or
@@ -21,6 +21,7 @@
 #pragma once
 #include "dm_device.cuh"
 #include "dm_kernels_index.cuh"      // K_A, dm_pdl_wait
+#include "dm_kernels_records.cuh"    // DmMonitors, dm_combo_seed / dm_combo_fold: combination monitors (dm_set_combos)
 
 #define DM_FMT_MAX_CHAINS 64          // log_format + 63 templates
 #define DM_FMT_MAX_LITS 512           // literals over all chains
@@ -232,8 +233,40 @@ __device__ __forceinline__ uint32_t dm_fmtl_normalise(const DmFormat& f, const u
     return o - s;
 }
 
+// Is monitor k present in this record, and where is its value?  Present exactly when the log_format matched (hok), the
+// record is in the monitor's event scope, and the header capture exists / the variable index is below the matched
+// template's wildcard count.  The value is cap = (offset, length) in `buf` for a header capture and for a variable
+// without R-norm; under R-norm a variable is a slice of the normalised copy `nbuf` (see dm_fmtl_value_fp).
+__device__ __forceinline__ bool dm_fmtl_locate(const DmFormat& f, uint32_t k, bool hok, int32_t eid, uint32_t n_hcaps,
+                                               uint32_t n_vars, const uint2* hcap, const uint2* vcap, uint2& cap) {
+    const uint32_t idx = f.mon_index[k];
+    bool use = hok && idx != DM_FMT_NONE && !(f.mon_has_event[k] && eid != f.mon_event[k]);
+    cap = make_uint2(0, 0);
+    if (use) {
+        if (f.mon_source[k]) {
+            use = eid >= 0 && idx < n_vars;
+            if (use) cap = vcap[(uint32_t)__popc(f.chain_need[eid + 1] & ((1u << idx) - 1u)) * DM_FMTL_THREADS];
+        } else {
+            use = idx < n_hcaps;
+            if (use) cap = hcap[(uint32_t)__popc(f.chain_need[0] & ((1u << idx) - 1u)) * DM_FMTL_THREADS];
+        }
+    }
+    return use;
+}
+
+// dm_fp64 of the value of monitor k that dm_fmtl_locate found
+template <bool NORM>
+__device__ __forceinline__ uint64_t dm_fmtl_value_fp(const DmFormat& f, uint32_t k, const uint8_t* buf, const uint8_t* nbuf,
+                                                     uint2 cap) {
+    return (NORM && f.mon_source[k]) ? dm_fmt_fp64<false>(nbuf, cap.x, cap.y) : dm_fmt_fp64<true>(buf, cap.x, cap.y);
+}
+
 // NORM: R-norm is configured; the templates then run on `nbuf`, the per-message normalised copy.
-template <bool TRAIN, bool NORM>
+// COMBO: combination monitors (a.combos is a DmMonitors, dm_set_combos; DESIGN.md R-combo): after the single
+// monitors, each combination folds the fingerprints of its members, re-hashed from the captures this lane keeps, into
+// one key under field n_mons + c.  Member-only monitors are not probed on their own.  (COMBO defaults to false, so
+// that `dm_k_format_lanes<TRAIN, NORM>` is the single-monitor kernel it always was.)
+template <bool TRAIN, bool NORM, bool COMBO = false>
 __global__ void __launch_bounds__(DM_FMTL_THREADS) dm_k_format_lanes(DmDetectArgs a, const DmFormat* __restrict__ gfmt,
                                                                      uint8_t* nbuf) {
     // [2][max_slots][DM_FMTL_THREADS]: header captures, template captures
@@ -269,6 +302,8 @@ __global__ void __launch_bounds__(DM_FMTL_THREADS) dm_k_format_lanes(DmDetectArg
     const uint64_t n_lines = a.hdr_in->n_lines;
     const uint64_t hi = a.line_hi < n_lines ? a.line_hi : n_lines;
     const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    const DmMonitors* __restrict__ cm = reinterpret_cast<const DmMonitors*>(a.combos);
+    const uint32_t member_only = COMBO ? cm->member_only : 0u;
 
     // the warps iterate a warp-uniform number of times; a lane without a record idles through the
     // same steps (see dm_fmtl_match_chain)
@@ -297,26 +332,34 @@ __global__ void __launch_bounds__(DM_FMTL_THREADS) dm_k_format_lanes(DmDetectArg
         }
         uint32_t unknown = 0;
         for (uint32_t k = 0; k < sf.n_mons; ++k) {
-            const uint32_t idx = sf.mon_index[k];
-            bool use = hok && idx != DM_FMT_NONE && !(sf.mon_has_event[k] && eid != sf.mon_event[k]);
-            uint2 cap = make_uint2(0, 0);
-            if (use) {
-                if (sf.mon_source[k]) {
-                    use = eid >= 0 && idx < n_vars;
-                    if (use) cap = vcap[(uint32_t)__popc(sf.chain_need[eid + 1] & ((1u << idx) - 1u)) * DM_FMTL_THREADS];
-                } else {
-                    use = idx < n_hcaps;
-                    if (use) cap = hcap[(uint32_t)__popc(sf.chain_need[0] & ((1u << idx) - 1u)) * DM_FMTL_THREADS];
-                }
-            }
-            if (use) {
-                const uint64_t fp = (NORM && sf.mon_source[k]) ? dm_fmt_fp64<false>(nbuf, cap.x, cap.y)
-                                                               : dm_fmt_fp64<true>(buf, cap.x, cap.y);
-                const uint64_t key = dm_make_key(fp, dm_field_salt(k));
+            if (COMBO && ((member_only >> k) & 1u)) continue;                  // (warp-uniform)
+            uint2 cap;
+            if (dm_fmtl_locate(sf, k, hok, eid, n_hcaps, n_vars, hcap, vcap, cap)) {
+                const uint64_t key = dm_make_key(dm_fmtl_value_fp<NORM>(sf, k, buf, nbuf, cap), dm_field_salt(k));
                 if (TRAIN) dm_table_insert(a.table, key, &a.hdr->error);
                 else if (!dm_table_contains(a.table, key)) unknown |= 1u << k;
             }
             __syncwarp();
+        }
+        if (COMBO) {
+            // combination c = ordered tuple of its members' values; yielded only when every member is present
+            for (uint32_t c = 0, n_combos = cm->n_combos; c < n_combos; ++c) {
+                const uint32_t lo = cm->combo_off[c], hi_m = cm->combo_off[c + 1];
+                uint64_t acc = dm_combo_seed(hi_m - lo);
+                bool all = true;
+                for (uint32_t j = lo; j < hi_m && all; ++j) {
+                    const uint32_t k = cm->combo_members[j];
+                    uint2 cap;
+                    all = dm_fmtl_locate(sf, k, hok, eid, n_hcaps, n_vars, hcap, vcap, cap);
+                    if (all) acc = dm_combo_fold(acc, dm_fmtl_value_fp<NORM>(sf, k, buf, nbuf, cap));
+                }
+                if (all) {
+                    const uint64_t key = dm_make_key(acc ? acc : 1ull, dm_field_salt(sf.n_mons + c));
+                    if (TRAIN) dm_table_insert(a.table, key, &a.hdr->error);
+                    else if (!dm_table_contains(a.table, key)) unknown |= 1u << (sf.n_mons + c);
+                }
+                __syncwarp();
+            }
         }
         if (!act) continue;
         if (!hok) atomicAdd(&s_bad, 1ull);

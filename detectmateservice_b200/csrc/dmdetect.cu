@@ -397,8 +397,6 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     if (nbytes == 0) DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
     h->last_nbytes = nbytes;
 
-    if (h->fmt_set && h->mons_set && h->h_mons.n_combos > 0)
-        return dm_fail(DM_ERR_STATE, "combination monitors are not evaluated in log_format mode (use key=value records or ParserSchema input)");
     if (h->fmt_set) {
         // log_format / template mode: K_A writes the record index, then one THREAD per record
         const uint32_t n_rows = (uint32_t)((nbytes + DMR_ROW - 1) / DMR_ROW);
@@ -419,7 +417,10 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
             DmDetectArgs a;
             a.buf = d_buf; a.line_start = h->d_line_start; a.hdr_in = h->d_hdr; a.hdr = h->d_hdr;
             a.keys = h->d_keys; a.table = h->table; a.flags = d_flags; a.scores = d_scores; a.out_cap = out_cap;
-            a.anomalies = h->d_anoms; a.anomaly_cap = h->anomaly_cap; a.stats = h->d_stats; a.nbytes = nbytes; a.combos = nullptr;
+            a.anomalies = h->d_anoms; a.anomaly_cap = h->anomaly_cap; a.stats = h->d_stats; a.nbytes = nbytes;
+            // combination monitors: the COMBO instantiations re-hash their members from the captures the lanes keep
+            const bool combos = h->mons_set && h->h_mons.n_combos > 0;
+            a.combos = combos ? (const void*)h->d_mons : nullptr;
             const uint64_t max_recs = std::min<uint64_t>(nbytes / 2 + 1, h->max_lines);
             const uint64_t want = (max_recs + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS;
             const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * 32));
@@ -427,13 +428,15 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
             const bool norm = h->fmt_norm != 0;
             if (n_train_lines > 0) {
                 a.line_lo = 0; a.line_hi = n_train_lines;
-                dm_launch_pdl_smem(norm ? dm_k_format_lanes<true, true> : dm_k_format_lanes<true, false>, (unsigned)grid,
-                                   DM_FMTL_THREADS, smem, st, false, a, (const DmFormat*)h->d_fmt, h->d_norm);
+                auto k = combos ? (norm ? dm_k_format_lanes<true, true, true> : dm_k_format_lanes<true, false, true>)
+                                : (norm ? dm_k_format_lanes<true, true, false> : dm_k_format_lanes<true, false, false>);
+                dm_launch_pdl_smem(k, (unsigned)grid, DM_FMTL_THREADS, smem, st, false, a, (const DmFormat*)h->d_fmt, h->d_norm);
             }
             a.line_lo = n_train_lines; a.line_hi = ~0ull;
             dm_prof_mark(h, st, 0);
-            dm_launch_pdl_smem(norm ? dm_k_format_lanes<false, true> : dm_k_format_lanes<false, false>, (unsigned)grid,
-                               DM_FMTL_THREADS, smem, st, false, a, (const DmFormat*)h->d_fmt, h->d_norm);
+            auto k = combos ? (norm ? dm_k_format_lanes<false, true, true> : dm_k_format_lanes<false, false, true>)
+                            : (norm ? dm_k_format_lanes<false, true, false> : dm_k_format_lanes<false, false, false>);
+            dm_launch_pdl_smem(k, (unsigned)grid, DM_FMTL_THREADS, smem, st, false, a, (const DmFormat*)h->d_fmt, h->d_norm);
             dm_prof_mark(h, st, 1);
             h->launches += 2 + (n_train_lines > 0 ? 1 : 0);
         }

@@ -164,9 +164,14 @@ int dm_set_monitors(dm_handle* h, uint32_t n_monitors, const dm_monitor_t* monit
  * field n_monitors + c and reported in bit n_monitors + c of the masks of
  * dm_process_records (n_monitors + n_combos <= 32).  Monitors whose bit is set in
  * member_only_mask do not alert on their own.  Call after dm_set_monitors (which clears the
- * combinations).  Applies to dm_process_records and to dm_process_lines on key=value records
+ * combinations).  Applies to dm_process_records, to dm_process_lines on key=value records
  * (monitor k = field k of dm_create; the library then uses its one-thread-per-record kernel,
- * dm_get_anomalies reports the same mask bits); not to log_format mode or the pipelined path. */
+ * dm_get_anomalies reports the same mask bits) and to dm_process_lines in log_format mode
+ * (dm_set_format[_ex], before or after this call): a member is present when the same monitor
+ * would be scored on its own -- the log_format matched, the record is in scope, the capture
+ * exists / the variable index is below the matched template's wildcard count; an empty
+ * capture is present.  Under R-norm a variable member's value is its slice of the normalised
+ * Content.  The key of a tuple is the same in all three modes.  Not the pipelined path. */
 int dm_set_combos(dm_handle* h, uint32_t n_combos, const uint32_t* member_off, const uint32_t* members,
                   uint32_t member_only_mask);
 /* MatcherParser fused in front of the detector (SURVEY.md section 8f-3).  Replaces
