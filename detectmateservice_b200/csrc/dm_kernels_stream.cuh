@@ -11,12 +11,13 @@
 //     flight, and every later access to the text (key bytes in front of an '=', the value behind
 //     it) is a shared-memory read at any alignment;
 //   * row phase (32 bytes per lane): count '\n' (for the record index, see epilogue), flag the '='
-//     bytes with SIMD-in-register compares into one 32-bit mask per lane, and look each of them up
-//     right there, in the lane that found it: the 4 bytes in front of the '=' index a perfect-hash
-//     table of the monitored keys' last four bytes (3-byte keys: delimiter + key).  Only hits --
-//     about as many as there are monitored fields, a quarter of the '=' -- go to the per-warp field
-//     queue, each lane's in byte order behind those of the lanes in front of it (one prefix over
-//     the lanes per round of at most four '=' per lane);
+//     bytes with SIMD-in-register compares into one byte-ordered 32-bit mask per lane, rank every '='
+//     of the row across the warp (a prefix of the lanes' counts: rank order = message order), and
+//     look them up by rank, 32 per step, so that the row's '=' are spread evenly over the lanes (the
+//     ranks go through a small per-warp array in shared memory, 128 per round): the 4 bytes in front
+//     of the '=' index a perfect-hash table of the monitored keys' last four bytes (3-byte keys:
+//     delimiter + key).  Only hits -- about as many as there are monitored fields, a quarter of the
+//     '=' -- go to the per-warp field queue, in rank order (one ballot per step);
 //   * field phase (one queued field per lane, 32 at a time): finish the key compare (bytes 5..12
 //     in front of the '=' and the field-start delimiter), find the value's end from ONE byte
 //     class ("stop bytes" < 0x23: space, '"', '\n', controls) over a 32-byte window, dm_fp64,
@@ -51,6 +52,7 @@
 #define DMX_WARPS 2
 #endif
 #define DMX_THREADS (DMX_WARPS * 32)
+#define DMX_ROUND 128u                      // '=' of a row looked up per round (4 per lane)
 #define DMX_QCAP 256u                       // field queue entries per warp (circular; a round adds at most 128 to at most 31)
 #define DMX_DEPTH 1u                        // rows loaded ahead (queued fields may then be up to 3 rows old)
 #define DMX_L1 512u                         // most slots of the level-1 key table
@@ -423,12 +425,14 @@ __device__ __forceinline__ bool dmx_verify_thread(const uint8_t* __restrict__ bu
 // state behind the last entry is carried to the next batch (DmxCarry): a long record is walked once,
 // not once per candidate.
 //
-// What the queue guarantees: entries are in message order, except in rows in which a lane holds more
-// than four '=' (`dense` rows): a round looks up at most four '=' per lane, so the rest of such a lane's
-// come behind the whole row's first round.  Batches that hold an entry of a dense row fall back to
-// dmx_verify_thread, which is always exact.  Every other batch is in order, and everything in front of
-// its first entry has left the queue: that is what the history (no carried state) or the carried state
-// stands for, and nothing still queued lies in front of any of its entries.
+// What the queue guarantees: entries are in message order, in every row (the row phase enqueues a row's
+// hits in the rank order of their '=', rounds and rows one after the other).  So everything in front of a
+// batch's first entry has left the queue: that is what the history (no carried state) or the carried state
+// stands for, and nothing still queued lies in front of any of its entries.  Batches that hold an entry of
+// a row in which a lane has more than four '=' (`dense` rows) still go to dmx_verify_thread as a whole.
+// Order no longer needs that; it keeps the always-exact one-by-one re-check running inside chained
+// streams, where the emulator tier compares the two on the same batches
+// (tests/test_emu_tile.py::test_emu_lookalikes_and_duplicates counts them).
 // ---------------------------------------------------------------------------------------
 // (inlined: as a real call the function's own register demand counts against the kernel's 64 and ptxas spills in the
 // row loop; inlined the rare path costs the detect kernel nothing)
@@ -444,7 +448,7 @@ struct DmxCarry {
     uint32_t ls;             // first byte of the record it lies in
     uint32_t par;            // quote parity at last_q
     uint32_t seen;           // keys of the true fields of that record up to and including last_q
-    int dense_row;           // last row (of this warp's) in which a lane had more than four '=': its entries are out of order
+    int dense_row;           // last row (of this warp's) in which a lane had more than four '=' (see above)
 };
 
 // bytes [lb, q): offset behind the last '\n' (found) and the parity of '"' behind it (else of the whole interval)
@@ -650,18 +654,38 @@ __device__ __forceinline__ uint32_t dmx_chunk_bits(const uint4& v, uint32_t pat)
     return (f0 >> 7) | (f1 >> 6) | (f2 >> 5) | (f3 >> 4);
 }
 
-// The same for '=' with the three-instruction zero-byte test, which is exact except that a run of '<' (0x3C = '=' ^ 1)
-// right behind an '=' in the same 32-bit word is flagged as well (the borrow of the subtraction).  Harmless: the bytes
-// in front of such a position hold that '=' within the last three, an '=' is part of no monitored key (dm_create rejects
-// it) and is no field-start delimiter, so the key lookup of the position fails like that of any other '=' that ends no
-// monitored key.  ('\n' is counted, so it keeps the exact test.)
+// The '=' of a 16-byte chunk IN BYTE ORDER (bit i = byte i: the set bits enumerate them in message order), with the
+// three-instruction zero-byte test, which is exact except that a run of '<' (0x3C = '=' ^ 1) right behind an '=' in the
+// same 32-bit word is flagged as well (the borrow of the subtraction).  Harmless: the bytes in front of such a position
+// hold that '=' within the last three, an '=' is part of no monitored key (dm_create rejects it) and is no field-start
+// delimiter, so the key lookup of the position fails like that of any other '=' that ends no monitored key.  ('\n' is
+// counted, so it keeps the exact test.)
 __device__ __forceinline__ uint32_t dmx_loose_bits(const uint4& v, uint32_t pat) {
     const uint32_t x0 = v.x ^ pat, x1 = v.y ^ pat, x2 = v.z ^ pat, x3 = v.w ^ pat;
     const uint32_t f0 = (x0 - 0x01010101u) & ~x0 & 0x80808080u, f1 = (x1 - 0x01010101u) & ~x1 & 0x80808080u;
     const uint32_t f2 = (x2 - 0x01010101u) & ~x2 & 0x80808080u, f3 = (x3 - 0x01010101u) & ~x3 & 0x80808080u;
-    return (f0 >> 7) | (f1 >> 6) | (f2 >> 5) | (f3 >> 4);
+    return dm_flags_to_nib(f0) | (dm_flags_to_nib(f1) << 4) | (dm_flags_to_nib(f2) << 8) | (dm_flags_to_nib(f3) << 12);
 }
 __device__ __forceinline__ uint32_t dmx_eq_bits(const uint4& v) { return dmx_loose_bits(v, 0x3D3D3D3Du); }
+
+// Inclusive prefix sum over the lanes of a warp.  (The shuffle's own "source lane exists" predicate guards each add,
+// so no lane index compare is issued per step.)
+__device__ __forceinline__ uint32_t dmx_warp_incl_sum(uint32_t v) {
+#pragma unroll
+    for (uint32_t d = 1; d < 32u; d <<= 1) {
+#ifndef DM_EMU
+        asm("{\n\t.reg .u32 t;\n\t.reg .pred p;\n\t"
+            "shfl.sync.up.b32 t|p, %0, %1, 0, -1;\n\t"
+            "@p add.u32 %0, %0, t;\n\t}"
+            : "+r"(v)
+            : "r"(d));
+#else
+        const uint32_t y = __shfl_up_sync(0xffffffffu, v, d);
+        if ((threadIdx.x & 31) >= d) v += y;
+#endif
+    }
+    return v;
+}
 template <bool TRAIN>
 __device__ __forceinline__ void dmx_epilogue(const DmxArgs& a, unsigned long long* s_pre);
 
@@ -819,6 +843,7 @@ __global__ void __launch_bounds__(DMX_THREADS, DMX_MIN_CTAS) dm_k_stream(DmxArgs
     // dynamic shared memory: DMX_WARPS rings, then the key table up to its last level-1 slot
     const DmxKeyTab& sk = *reinterpret_cast<const DmxKeyTab*>(s_dyn + a.ring_smem);
     __shared__ uint32_t s_q[DMX_WARPS][DMX_QCAP];
+    __shared__ uint16_t s_eq[DMX_WARPS][DMX_ROUND];
     __shared__ unsigned long long s_bar[DMX_WARPS][DMX_SLOTS];
     __shared__ uint32_t s_cnt[DMX_WARPS];
     __shared__ unsigned long long s_bound;
@@ -900,6 +925,7 @@ __global__ void __launch_bounds__(DMX_THREADS, DMX_MIN_CTAS) dm_k_stream(DmxArgs
         const uint32_t tail_bytes = (uint32_t)(nbytes & (DMX_ROW - 1));   // valid bytes of a partial last row (0 = full)
         const uint32_t tail_row = tail_bytes ? a.n_rows - 1 : 0xFFFFFFFFu;
         uint32_t* q = s_q[warp];                               // fields waiting for the field phase: (offset in this warp's range << 7) | level-1 info
+        uint16_t* eq = s_eq[warp];                             // the '=' of a lookup round by rank: offset in the row
         uint32_t qh = 0, qn = 0, nl_w = 0;
         if (rg.r0 == 0) {
             // a message starts a record: the 16 bytes "in front of it" read as '\n'
@@ -941,53 +967,53 @@ __global__ void __launch_bounds__(DMX_THREADS, DMX_MIN_CTAS) dm_k_stream(DmxArgs
                 if (lane == 0) a.row_cnt[row] = (unsigned short)tot;
                 nl_w += tot;
             }
-            // the '=' of this lane's 32 bytes: bit 8b + 4c + w = byte b of word w of chunk c
-            uint32_t g = (dmx_eq_bits(va) << (4u * c_first)) | (dmx_eq_bits(vb) << (4u * (1u - c_first)));
-            const uint32_t qrel = i * DMX_ROW + lane * 32u;
+            // the '=' of this lane's 32 bytes: bit i = byte i
+            uint32_t g = (dmx_eq_bits(va) << (16u * c_first)) | (dmx_eq_bits(vb) << (16u * (1u - c_first)));
+            const uint32_t cnt = (uint32_t)__popc(g);
             const bool last = i + 1 == n_own;
             if (CHAIN) {
-                if (__any_sync(0xffffffffu, __popc(g) > 4)) {       // (see dmx_verify_chain)
+                if (__any_sync(0xffffffffu, cnt > 4u)) {            // (see dmx_verify_chain)
                     if (lane == 0) s_carry[warp].dense_row = (int)i;
                     __syncwarp();
                 }
             }
+            // rank of this lane's first '=' among the row's (message order): exclusive prefix of the lanes' counts
+            uint32_t rank = dmx_warp_incl_sum(cnt);
+            const uint32_t n_eq = __shfl_sync(0xffffffffu, rank, 31);
+            rank -= cnt;
+            const uint32_t rb = (row & (DMX_SLOTS - 1)) * DMX_SLOT + DMX_PRE;          // the row in the ring
+            uint32_t r_lo = 0;                                                        // first rank of the round
             bool row_done;
             do {
-                // ---- level-1 lookup of up to 4 of this lane's '=' per round: the 4 bytes in front of each (shared
-                // memory, any alignment) -> perfect-hash table; a hit becomes a field queue entry ----
+                // ---- ranks [r_lo, r_lo + DMX_ROUND): offsets in the row -> s_eq[rank - r_lo].  Lane j then looks up
+                // ranks j, j + 32, ... of the round: the 4 bytes in front of the '=' (shared memory, any alignment)
+                // -> perfect-hash table; the hits go to the field queue in rank order, i.e. in message order ----
                 {
-                    const uint32_t have = (uint32_t)__popc(g);
-                    const uint32_t cnt = have < 4u ? have : 4u;
-                    uint32_t e[4];
+                    while (g && rank < r_lo + DMX_ROUND) {
+                        eq[rank - r_lo] = (uint16_t)(lane * 32u + (uint32_t)__ffs(g) - 1u);
+                        g &= g - 1u;
+                        ++rank;
+                    }
+                    __syncwarp();
+                    const uint32_t nr = n_eq - r_lo < DMX_ROUND ? n_eq - r_lo : DMX_ROUND;
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        e[j] = 0xFFFFFFFFu;
-                        if ((uint32_t)j < cnt) {
-                            const uint32_t x = (uint32_t)__ffs(g) - 1u;
-                            g &= g - 1u;
-                            const uint32_t off = ((x & 7u) << 2) + (x >> 3);      // of the '=' in the lane's 32 bytes
-                            const uint32_t at = lb + off - 4u;
+                    for (uint32_t s = 0; s < DMX_ROUND / 32u; ++s) {
+                        if (32u * s >= nr) break;
+                        uint32_t off = 0, info = 0;
+                        if (32u * s + lane < nr) {
+                            off = eq[32u * s + lane];
+                            const uint32_t at = rb + off - 4u;
                             const uint32_t t = __funnelshift_r(dmx_ld32(ring, at & ~3u), dmx_ld32(ring, (at & ~3u) + 4u), (at & 3u) * 8u);
                             const DmxL1 l = sk.l1[(t * l1_mult) >> l1_shift];
-                            uint32_t info = l.pat == t ? l.info : 0u;
+                            info = l.pat == t ? l.info : 0u;
                             if (!info && n_short) info = dmx_short_key(t, sk, a.keys);
-                            if (info) e[j] = ((qrel + off) << 7) | info;
                         }
+                        const uint32_t hit = __ballot_sync(0xffffffffu, info != 0u);
+                        if (info) q[(qh + qn + (uint32_t)__popc(hit & lt)) & (DMX_QCAP - 1)] = ((i * DMX_ROW + off) << 7) | info;
+                        qn += (uint32_t)__popc(hit);
                     }
-                    // the lane's hits in byte order (entries grow with the offset; misses sort behind them), then behind
-                    // those of the lanes in front of it: the queue stays in message order except in dense rows
-#define DMX_CSWAP(i, j) { const uint32_t lo_ = e[i] < e[j] ? e[i] : e[j]; e[j] = e[i] < e[j] ? e[j] : e[i]; e[i] = lo_; }
-                    DMX_CSWAP(0, 1) DMX_CSWAP(2, 3) DMX_CSWAP(0, 2) DMX_CSWAP(1, 3) DMX_CSWAP(1, 2)
-#undef DMX_CSWAP
-                    const uint32_t nh = (e[0] != 0xFFFFFFFFu) + (e[1] != 0xFFFFFFFFu) + (e[2] != 0xFFFFFFFFu) + (e[3] != 0xFFFFFFFFu);
-                    const uint32_t b0 = __ballot_sync(0xffffffffu, nh & 1u), b1 = __ballot_sync(0xffffffffu, nh & 2u);
-                    const uint32_t b2 = __ballot_sync(0xffffffffu, nh & 4u);
-                    const uint32_t slot = qh + qn + (uint32_t)__popc(b0 & lt) + 2u * (uint32_t)__popc(b1 & lt) + 4u * (uint32_t)__popc(b2 & lt);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        if ((uint32_t)j < nh) q[(slot + j) & (DMX_QCAP - 1)] = e[j];
-                    qn += (uint32_t)__popc(b0) + 2u * (uint32_t)__popc(b1) + 4u * (uint32_t)__popc(b2);
-                    row_done = !__any_sync(0xffffffffu, g != 0u);
+                    r_lo += DMX_ROUND;
+                    row_done = r_lo >= n_eq;
                     __syncwarp();
                 }
                 // ---- full passes; at the end of a row also whatever is left of rows up to (i + 2 - SLOTS): the next
