@@ -15,8 +15,8 @@ UNMODIFIED reference service:
                   data_use_training, auto_config, global: {...}, events: {...}, params: {...}}}``;
                   GPU options live under ``params`` (settings.py has extra="forbid").
 
-Two input formats, told apart per message (``params.input_format``: auto | raw_lines |
-parser_schema):
+Input formats, told apart per message (``params.input_format``: auto | raw_lines |
+parser_schema | parser_schema_batch), or named (log_schema | log_schema_batch, never chosen by auto):
 
   record mode   one serialized ParserSchema per message -- what the upstream parser stage
                 sends today.  The host decodes the protobuf framing, the monitored values go
@@ -28,6 +28,10 @@ parser_schema):
                 records (a single bare message when the input held one record, else
                 varint-length-delimited), None when there are none; ``compact`` =
                 ``<u32 n><n x u8 flag><n x f32 score>`` for pipelines that want every score.
+  LogSchema     what the reader stage sends (one serialized LogSchema per message, or a delimited
+                batch): the device unwraps each record's ``log`` text and runs raw-mode detection on
+                it, so that with a ``log_format`` this component stands where the parser stands.
+                Replies as for ParserSchema input; alerts carry the record's logID.
 
 All detection decisions are taken on the device; there is no CPU path (DeviceDetector
 raises without a GPU).
@@ -116,6 +120,11 @@ def parse_monitors(cfg: dict) -> List[Monitor]:
     return mons
 
 
+# log_schema / log_schema_batch are opt-in: protobuf's runtime parses any LogSchema as a ParserSchema (the string fields
+# 1, 2, 3 and 5 are ParserSchema strings too), so `auto` cannot tell the two apart and keeps reading ParserSchema.
+INPUT_FORMATS = ("auto", "raw_lines", "parser_schema", "parser_schema_batch", "log_schema", "log_schema_batch")
+
+
 class B200NewValueDetector(CoreComponent):
     accepts_bytes_like = True      # process() takes bytes, bytearray or memoryview (see service.py)
 
@@ -134,8 +143,8 @@ class B200NewValueDetector(CoreComponent):
         self.start_id = int(cfg.get("start_id", 10))
         self.input_format = cfg.get("input_format", "auto")
         self.output_format = cfg.get("output_format", "alerts")
-        if self.input_format not in ("auto", "raw_lines", "parser_schema", "parser_schema_batch"):
-            raise ValueError(f"input_format {self.input_format!r} not in auto|raw_lines|parser_schema|parser_schema_batch")
+        if self.input_format not in INPUT_FORMATS:
+            raise ValueError(f"input_format {self.input_format!r} not in {'|'.join(INPUT_FORMATS)}")
         if self.output_format not in ("alerts", "compact"):
             raise ValueError(f"output_format {self.output_format!r} not in alerts|compact")
         self.monitors = parse_monitors(cfg)
@@ -283,6 +292,8 @@ class B200NewValueDetector(CoreComponent):
             return self._process_record(data)
         if fmt == "parser_schema_batch":
             return self._process_record_batch(data)
+        if fmt in ("log_schema", "log_schema_batch"):
+            return self._process_logs(data, delimited=fmt == "log_schema_batch")
         return self._process_lines(data)
 
     # ------------------------------------------------------------------ record mode
@@ -354,6 +365,44 @@ class B200NewValueDetector(CoreComponent):
             t = (rec.get("logFormatVariables") or {}).get("Time")
             out.append(self._detector_schema(rec.get("logID", ""), float(scores[idx]), alerts, t))
         return wire.frame_delimited(out) if out else None
+
+    # ------------------------------------------------------------------ LogSchema input (the reader stage's records)
+    def _process_logs(self, data: bytes, delimited: bool) -> Optional[bytes]:
+        """One bare LogSchema record, or a length-delimited batch of them: the device unwraps each record's `log` text
+        and detects it as a raw line (key=value, or the log_format).  Replies as for ParserSchema input; the alert of a
+        record carries its logID.  A malformed bare record raises WireError and takes no training slot."""
+        if len(data) > self.max_batch_bytes:
+            raise ValueError(f"a LogSchema message of {len(data)} bytes exceeds max_batch_bytes={self.max_batch_bytes}")
+        remaining = max(0, self.data_use_training - self.n_seen)
+        try:
+            flags, scores, n_bad = self.det.process_logs(data, n_train_records=remaining, delimited=delimited)
+        except Exception as e:
+            self._count_dropped_training(e, remaining, lambda: len(wire.split_delimited(data)) if delimited else 1)
+            raise
+        n = int(flags.size)
+        self.last_n_malformed = n_bad
+        self.n_seen += n - n_bad                                 # malformed and unusable records take no training slot
+        if not delimited and n_bad:
+            raise wire.WireError("malformed LogSchema record")
+        if self.output_format == "compact":
+            return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
+        if self.det.last_n_anomalies == 0:
+            return None
+        frames = wire.split_delimited(data) if delimited else [data]
+        raw_keys = [m.key for m in self.monitors]
+        out = []
+        for idx, mask, _offset in self.det.anomalies():
+            rec = wire.decode_log_schema(frames[idx])
+            line = wire.log_schema_line(rec)
+            if self.logformat is not None:
+                _eid, variables, lfv = self.logformat.parse(line) or (-1, [], {})
+                alerts, t = self._format_alerts(variables, lfv, mask), lfv.get("Time")
+            else:
+                alerts, t = self._line_alerts(line, mask, raw_keys), _alerts.record_time(line)
+            out.append(self._detector_schema(rec["logID"], float(scores[idx]), alerts, t))
+        if not out:
+            return None
+        return wire.frame_delimited(out) if delimited else out[0]
 
     # ------------------------------------------------------------------ raw mode
     def _process_lines(self, data: bytes) -> Optional[bytes]:

@@ -17,6 +17,7 @@
 #include "dm_kernels_stream.cuh"
 #include "dm_kernels_values.cuh"
 #include "dm_kernels_records.cuh"
+#include "dm_kernels_logs.cuh"
 #include "dm_kernels_format.cuh"
 #include "dm_kernels_lanes.cuh"
 #include "dm_format_host.h"
@@ -101,6 +102,14 @@ struct dm_handle {
     uint64_t win_seq = 0;
     bool fmt_set = false;
     uint32_t fmt_slots = 1;        // DmFormat.max_slots (dynamic shared memory of the thread-per-record kernel)
+    // LogSchema input (dm_process_logs), allocated on first use
+    uint8_t* d_logs_text = nullptr;      // the compacted texts + slack
+    uint64_t logs_text_cap = 0;
+    void* d_logs = nullptr;              // per-record / per-line / per-chunk arrays of DmLogsArgs
+    uint64_t logs_cap = 0;               // records they hold
+    uint32_t logs_chunks = 0;            // chunks they hold
+    DmLogsHeader* d_lhdr = nullptr;
+    DmLogsHeader* h_lhdr = nullptr;      // pinned
     // pipelined host path: two slots
     struct Slot {
         uint8_t* d_in = nullptr; uint8_t* d_flags = nullptr; float* d_scores = nullptr;
@@ -312,6 +321,7 @@ extern "C" int dm_destroy(dm_handle* h) {
     cudaFreeHost(h->h_hdr); cudaFreeHost(h->h_err); cudaFree(h->d_anoms); cudaFree(h->d_stats); cudaFreeHost(h->h_stats);
     cudaFree(h->table.slots); cudaFree(h->table.novel); cudaFree(h->table.count);
     cudaFree(h->d_vals); cudaFree(h->d_masks); cudaFree(h->d_mons); cudaFree(h->d_fmt); cudaFree(h->d_norm);
+    cudaFree(h->d_logs_text); cudaFree(h->d_logs); cudaFree(h->d_lhdr); cudaFreeHost(h->h_lhdr);
     for (int k = 0; k < 2; ++k) {
         cudaFree(h->d_win[k]);
         if (h->ev_win_done[k]) cudaEventDestroy(h->ev_win_done[k]);
@@ -762,6 +772,146 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     int rc = dm_check_device_errors(h);
     if (rc != DM_OK) return rc;
     if (n_records_out) *n_records_out = n_records;
+    if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    return DM_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// LogSchema input (the reader stage's records): unwrapped on the device, then the line path
+// ---------------------------------------------------------------------------------------
+// The compacted texts need at most max_batch_bytes + 1 bytes, whatever the batch: every record spends at least len + 1
+// bytes of the caller's message on a text of len bytes -- the text plus its length prefix, or (a bare record) plus
+// the `log` field's tag and length -- except a bare record of zero bytes, which compacts to a single '\n'.  The slack
+// the line kernels read past the end, and the rounding to whole 16-byte stores, come on top.  So one buffer, allocated
+// on the first call, serves every call.  The per-record arrays grow with the largest batch seen.
+static int dm_logs_reserve(dm_handle* h, uint64_t n_records, uint32_t n_chunks) {
+    if (!h->d_lhdr) {
+        DM_CUDA(cudaMalloc(&h->d_lhdr, sizeof(DmLogsHeader)));
+        DM_CUDA(cudaHostAlloc(&h->h_lhdr, sizeof(DmLogsHeader), cudaHostAllocDefault));
+        h->logs_text_cap = (h->max_batch_bytes + 1 + DML_SLACK + 15) & ~15ull;
+        DM_CUDA(cudaMalloc(&h->d_logs_text, h->logs_text_cap));
+    }
+    if (n_records <= h->logs_cap && n_chunks <= h->logs_chunks) return DM_OK;
+    const uint64_t cap = std::min<uint64_t>(std::max<uint64_t>({n_records, 2 * h->logs_cap, 4096}), h->max_lines);
+    const uint32_t chunks = std::max<uint32_t>(n_chunks, (uint32_t)h->sm_count * 4);
+    if (h->d_logs) DM_CUDA(cudaFree(h->d_logs));
+    h->d_logs = nullptr;
+    h->logs_cap = 0;
+    // loc + chunk (u64), 8 u32 arrays of cap + 1, scores (f32), flags (u8)
+    DM_CUDA(cudaMalloc(&h->d_logs, 8 * (cap + chunks) + 4 * 8 * (cap + 1) + 4 * cap + cap + 16));
+    h->logs_cap = cap;
+    h->logs_chunks = chunks;
+    return DM_OK;
+}
+
+// The arrays of dm_logs_reserve, carved out of one allocation.
+static DmLogsArgs dm_logs_args(dm_handle* h, float** scores, uint8_t** flags) {
+    DmLogsArgs a;
+    const uint64_t cap = h->logs_cap;
+    unsigned long long* w = (unsigned long long*)h->d_logs;
+    a.loc = w;
+    a.chunk = w + cap;
+    uint32_t* u = (uint32_t*)(w + cap + h->logs_chunks);
+    uint32_t* arr[8];
+    for (int i = 0; i < 8; ++i) arr[i] = u + (uint64_t)i * (cap + 1);
+    a.rec_off = arr[0]; a.rec_len = arr[1]; a.text_off = arr[2]; a.text_len = arr[3];
+    a.rec_line = arr[4]; a.line_src = arr[5]; a.line_dst = arr[6]; a.line_rec = arr[7];
+    *scores = (float*)(u + 8 * (cap + 1));
+    *flags = (uint8_t*)(*scores + cap);
+    a.out = h->d_logs_text;
+    a.out_cap = h->logs_text_cap;
+    a.lhdr = h->d_lhdr;
+    return a;
+}
+
+extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimited, uint32_t n_train_records,
+                               uint8_t* flags_out, float* scores_out, uint64_t out_cap,
+                               uint64_t* n_records_out, uint64_t* n_malformed_out, uint64_t* n_anomalies_out) {
+    if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
+    if (nbytes && !buf) return dm_fail(DM_ERR_ARG, "buf is NULL");
+    if (nbytes > h->max_batch_bytes) return dm_fail(DM_ERR_CAPACITY, "message of %llu bytes exceeds max_batch_bytes=%llu", (unsigned long long)nbytes, (unsigned long long)h->max_batch_bytes);
+    // framing: one bare record, or varint length, payload, varint length, payload ...
+    std::vector<uint32_t> off, len;
+    if (!delimited) {
+        off.push_back(0);
+        len.push_back((uint32_t)nbytes);
+    }
+    uint64_t pos = 0;
+    while (delimited && pos < nbytes) {
+        uint64_t l = 0;
+        int shift = 0;
+        for (;;) {
+            if (pos >= nbytes || shift > 63) return dm_fail(DM_ERR_ARG, "truncated length prefix at byte %llu", (unsigned long long)pos);
+            const uint8_t b = buf[pos++];
+            l |= (uint64_t)(b & 0x7F) << shift;
+            if (!(b & 0x80)) break;
+            shift += 7;
+        }
+        if (l > nbytes - pos) return dm_fail(DM_ERR_ARG, "record of %llu bytes at byte %llu runs past the end of the message", (unsigned long long)l, (unsigned long long)pos);
+        off.push_back((uint32_t)pos);
+        len.push_back((uint32_t)l);
+        pos += l;
+    }
+    const uint32_t n_records = (uint32_t)off.size();
+    if (n_records > h->max_lines) return dm_fail(DM_ERR_CAPACITY, "%u records exceed max_lines=%llu", n_records, (unsigned long long)h->max_lines);
+    if ((flags_out || scores_out) && n_records > out_cap)
+        return dm_fail(DM_ERR_CAPACITY, "batch holds %u records, output capacity is %llu", n_records, (unsigned long long)out_cap);
+    DM_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    h->last_stream = st;
+    dm_break_chain(h, st);
+    // walk grid: at most 4 CTAs per SM, each a contiguous chunk of whole DML_THREADS-record tiles
+    const uint32_t tiles = (n_records + DML_THREADS - 1) / DML_THREADS;
+    const uint32_t want = std::max<uint32_t>(1, std::min<uint32_t>(tiles, (uint32_t)h->sm_count * 4));
+    const uint32_t per_cta = std::max<uint32_t>(1, (tiles + want - 1) / want) * DML_THREADS;
+    const uint32_t n_chunks = (n_records + per_cta - 1) / per_cta;
+    int rc = dm_logs_reserve(h, n_records, n_chunks);
+    if (rc != DM_OK) return rc;
+    float* d_rscores;
+    uint8_t* d_rflags;
+    DmLogsArgs a = dm_logs_args(h, &d_rscores, &d_rflags);
+    a.buf = h->d_in; a.n_records = n_records; a.n_train_records = n_train_records; a.per_cta = per_cta; a.n_chunks = n_chunks;
+    if (nbytes) DM_CUDA(cudaMemcpyAsync(h->d_in, buf, nbytes, cudaMemcpyHostToDevice, st));
+    if (n_records) {
+        DM_CUDA(cudaMemcpyAsync((void*)a.rec_off, off.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
+        DM_CUDA(cudaMemcpyAsync((void*)a.rec_len, len.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
+        const int grid_r = (int)std::min<uint32_t>(tiles, (uint32_t)h->sm_count * 8);
+        // the copy grid covers the largest compacted size this message can have (the total is not known yet)
+        const uint64_t stores = (std::max<uint64_t>(nbytes, 1) + DML_SLACK + 15) / 16;
+        const int grid_c = (int)std::min<uint64_t>((stores + DML_THREADS - 1) / DML_THREADS, (uint64_t)h->sm_count * 16);
+        dm_k_logs_walk<<<n_chunks, DML_THREADS, 0, st>>>(a);
+        dm_k_logs_scan<<<1, DML_THREADS, 0, st>>>(a);
+        dm_k_logs_compact<<<grid_r, DML_THREADS, 0, st>>>(a);
+        dm_k_logs_copy<<<grid_c, DML_THREADS, 0, st>>>(a);
+        h->launches += 4;
+        DM_CUDA(cudaGetLastError());
+    } else {
+        DM_CUDA(cudaMemsetAsync(h->d_lhdr, 0, sizeof(DmLogsHeader), st));
+    }
+    DM_CUDA(cudaMemcpyAsync(h->h_lhdr, h->d_lhdr, sizeof(DmLogsHeader), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
+    const DmLogsHeader lh = *h->h_lhdr;
+    if (lh.n_lines) {
+        uint64_t n_lines = 0, n_anoms = 0;
+        rc = dm_process_lines(h, h->d_logs_text, lh.total_bytes, 1, lh.n_train, nullptr, nullptr, 0, 0, &n_lines, &n_anoms, st);
+        dm_break_chain(h, st);
+        if (rc != DM_OK) return rc;
+        if (n_lines != lh.n_lines)
+            return dm_fail(DM_ERR_STATE, "the line path found %llu records in %llu unwrapped texts", (unsigned long long)n_lines, (unsigned long long)lh.n_lines);
+    } else {
+        DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+    }
+    const int grid_s = (int)std::max<uint32_t>(1, std::min<uint32_t>(std::max<uint32_t>(tiles, h->anomaly_cap / DML_THREADS), (uint32_t)h->sm_count * 8));
+    dm_k_logs_scatter<<<grid_s, DML_THREADS, 0, st>>>(a, h->d_flags, h->d_scores, d_rflags, d_rscores, h->d_anoms, h->anomaly_cap,
+                                                     h->d_hdr, h->d_stats, nbytes);
+    h->launches++;
+    DM_CUDA(cudaGetLastError());
+    DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
+    if (flags_out && n_records) DM_CUDA(cudaMemcpyAsync(flags_out, d_rflags, n_records, cudaMemcpyDeviceToHost, st));
+    if (scores_out && n_records) DM_CUDA(cudaMemcpyAsync(scores_out, d_rscores, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
+    if (n_records_out) *n_records_out = n_records;
+    if (n_malformed_out) *n_malformed_out = n_records - lh.n_lines;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
     return DM_OK;
 }

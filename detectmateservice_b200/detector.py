@@ -251,6 +251,23 @@ class DeviceDetector:
         k = n_rec.value
         return flags[:k], scores[:k], masks[:k]
 
+    def process_logs(self, buf: bytes, n_train_records: int = 0, delimited: bool = True
+                     ) -> Tuple[np.ndarray, np.ndarray, int]:
+        """LogSchema records -- one bare record (delimited=False) or a varint-length-delimited batch -- whose `log`
+        texts are unwrapped on the device and detected as raw lines (key=value, or the log_format of set_format).
+        The first n_train_records usable records train.  Returns (flags u8, scores f32, records malformed or
+        unusable), one flag and score per record; anomalies() then names records and their payload offsets."""
+        cap = max(1, len(buf)) if delimited else 1              # (a delimited record takes at least its length byte)
+        flags = np.empty(cap, dtype=np.uint8)                   # (the library writes the first n_records entries)
+        scores = np.empty(cap, dtype=np.float32)
+        n_rec, n_bad, n_anom = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        _lib.check(self._lib.dm_process_logs(self._h, bytes(buf), len(buf), int(bool(delimited)), int(n_train_records),
+                                             flags.ctypes.data, scores.ctypes.data, cap, C.byref(n_rec), C.byref(n_bad),
+                                             C.byref(n_anom)))
+        self.last_n_anomalies = n_anom.value
+        k = n_rec.value
+        return flags[:k], scores[:k], int(n_bad.value)
+
     def sync(self) -> Tuple[int, int]:
         n_lines = C.c_uint64()
         n_anom = C.c_uint64()

@@ -314,6 +314,54 @@ def decode_detector_schema(buf: bytes) -> Dict:
     return rec
 
 
+# LogSchema: what the reader stage sends; every field is a proto3 string
+_LOG_NAMES = {1: "__version__", 2: "logID", 3: "log", 4: "logSource", 5: "hostname"}
+
+
+def decode_log_schema(buf: bytes, strict: bool = False) -> Dict:
+    """LogSchema bytes -> dict of str (absent fields read as "").  Accepts exactly what protobuf's runtime accepts,
+    except that a group raises (as decode_parser_schema): invalid UTF-8 in fields 1-5, field 0, a tag of 2^32 or more,
+    or a payload running past the end raise WireError; the last occurrence of a field wins.  strict: unknown fields and
+    known fields under another wire type raise too; otherwise they are skipped like protobuf does."""
+    rec: Dict = {name: "" for name in _LOG_NAMES.values()}
+    pos, n = 0, len(buf)
+    while pos < n:
+        field, wt, pos = _read_tag(buf, pos)
+        if wt == 2 and (field in _LOG_NAMES or not strict):
+            ln, pos = _read_varint(buf, pos)
+            end = pos + ln
+            if end > n:
+                raise WireError("length-delimited field runs past the end")
+            if field in _LOG_NAMES:
+                rec[_LOG_NAMES[field]] = _utf8(buf[pos:end])
+            pos = end
+        elif strict:
+            raise WireError(f"unexpected wire type {wt} for field {field}")
+        else:
+            pos = _skip_field(buf, pos, n, wt)
+    return rec
+
+
+def log_schema_line(rec: Dict) -> bytes:
+    """The text a LogSchema record contributes as a raw line (DESIGN.md R-log): its `log` less one trailing '\\n'.
+    A text that still holds a '\\n' would be two lines: WireError, as for a malformed record."""
+    text = rec.get("log", "").encode("utf-8")
+    if text.endswith(b"\n"):
+        text = text[:-1]
+    if b"\n" in text:
+        raise WireError("LogSchema log holds more than one line")
+    return text
+
+
+def encode_log_schema(rec: Dict) -> bytes:
+    """dict -> LogSchema bytes (fields present in rec, in field order)."""
+    out = bytearray()
+    for field, name in _LOG_NAMES.items():
+        if name in rec:
+            _write_str(out, field, rec[name])
+    return bytes(out)
+
+
 def frame_delimited(messages: List[bytes]) -> bytes:
     """varint-length-delimited stream (protobuf's writeDelimitedTo framing)."""
     out = bytearray()

@@ -224,6 +224,26 @@ int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nbytes, uint32
                        uint8_t* flags_out, float* scores_out, uint32_t* masks_out, uint64_t out_cap,
                        uint64_t* n_records_out, uint64_t* n_anomalies_out);
 
+/* LogSchema input: what the reader stage sends (one serialized LogSchema per message), so that the detector -- with
+ * dm_set_format[_ex] the parser and the detector fused -- can stand where the parser service stands.
+ *   delimited = 0: buf is ONE bare LogSchema record; 1: varint-length-delimited records.
+ * Each record's text is unwrapped on the device and the texts go through dm_process_lines' detection unchanged
+ * (key=value or log_format mode, combinations included).  Rule R-log (DESIGN.md):
+ *   - a record is well-formed if and only if protobuf's runtime parses it as LogSchema (fields 1-5 are strings, strict
+ *     UTF-8 in all of them), with the same exception as dm_process_records: a group makes it malformed;
+ *   - its text is its `log` field (the last one wins; absent = "") less ONE trailing '\n'; a text that still holds a
+ *     '\n' is unusable;
+ *   - malformed and unusable records get flag and score 0, count in dm_stats_t.bad_records and take no training slot;
+ *   - every other record gets exactly the result its text gets as a line of a dm_process_lines message made of the
+ *     usable texts, each followed by '\n', in order; the first n_train_records of them train.
+ * flags_out / scores_out: host buffers of out_cap entries, one per record (either may be NULL).  *n_malformed_out =
+ * malformed + unusable records.  dm_get_anomalies then reports (record index, mask, byte offset of the record's payload
+ * in buf).  Statistics: lines += records, bytes += nbytes, train_lines / detect_lines as dm_process_records counts them.
+ * Synchronous; ends the overlap chain of dm_process_lines (dm_set_overlap).  Not the pipelined path. */
+int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimited, uint32_t n_train_records,
+                    uint8_t* flags_out, float* scores_out, uint64_t out_cap,
+                    uint64_t* n_records_out, uint64_t* n_malformed_out, uint64_t* n_anomalies_out);
+
 /* Pipelined host path (two slots): dm_submit_lines enqueues, without waiting, the copy of a
  * HOST message (pinned memory gives real overlap) to the device, the kernels and the copy
  * of the batch header back; dm_collect waits for that slot, copies the slot's flags and
