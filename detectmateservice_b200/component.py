@@ -171,6 +171,7 @@ class B200NewValueDetector(CoreComponent):
         self.n_seen = 0
         self.n_alerts = 0
         self.clock = time.time
+        self._alert_sig = None                 # (handle, detector_id, method_type) the device's alert format was set for
 
     # ------------------------------------------------------------------ device handle
     @property
@@ -239,6 +240,7 @@ class B200NewValueDetector(CoreComponent):
         if self._det is not None:
             self._det.close()
             self._det = None
+        self._alert_sig = None
 
     def reconfigure(self, config: Optional[Any]) -> bool:
         """Take a new detector configuration (what Service.reconfigure has just put into its config manager,
@@ -436,6 +438,13 @@ class B200NewValueDetector(CoreComponent):
     # scripts/e2e_pieces.py measures one call against 2 / 4 / 8 / 12 MiB pieces on the machine at hand.
     PIPE_MIN_BYTES = 24 << 20
     PIPE_PIECE_BYTES = 12 << 20
+    # Batches with at least this many anomalous records have their alerts encoded on the device (dm_encode_alerts).  On
+    # one H100 (700 W), 64k-record messages, process() median [range] in ms, host encoder against device encoder: 1 alert
+    # 0.60 against 0.59 [0.57-0.62], 4 alerts 0.65 [0.56-0.75] against 0.58 [0.55-0.61], 8 alerts 0.61 [0.59-0.76]
+    # against 0.54 [0.53-0.60], 16 alerts 0.92 against 0.58 (scripts/alerts_bench.py, DESIGN.md section 5.3).  Below 8
+    # the two overlap, and a record with a long value once made one alert slower on the device (0.77 against 0.60), so
+    # the device takes over where it was ahead beyond the spread.
+    DEVICE_ALERTS_MIN = 8
 
     def _detect_pipelined(self, data):
         """Detection-only message, key=value records: cut it at record boundaries into ~4 MiB pieces and run them
@@ -494,6 +503,17 @@ class B200NewValueDetector(CoreComponent):
             return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
         if n_anom == 0:
             return None
+        if anomalies is None and n_anom >= self.DEVICE_ALERTS_MIN:
+            enc = self._device_alerts(base, n)
+            if enc is not None:
+                blob, count = enc
+                self.n_alerts += count
+                if not count:
+                    return None
+                if n == 1 and not force_delimited:
+                    _ln, pos = wire._read_varint(blob, 0)              # one record in, one bare DetectorSchema out
+                    return blob[pos:]
+                return blob
         if anomalies is None:
             anomalies = self.det.anomalies()
         out = []
@@ -542,6 +562,35 @@ class B200NewValueDetector(CoreComponent):
                 for i in range(len(raw_keys)) if mask >> i & 1}
 
     # ------------------------------------------------------------------ output
+    def _alert_keys(self) -> List[Tuple[str, List[int]]]:
+        """alertsObtain keys in the order the host encoder writes them (sorted), each with the mask bits that supply it
+        in config order (two monitors may share a key: the last one flagged wins, as in _line_alerts)."""
+        by_key: Dict[str, List[int]] = {}
+        for i, m in enumerate(self.monitors):
+            by_key.setdefault(m.alert_key, []).append(i)
+        return sorted(by_key.items())
+
+    def _device_alerts(self, first_log_id: int, n_records: int) -> Optional[Tuple[bytes, int]]:
+        """The alerts of the last raw-line batch encoded on the device (DESIGN.md R-alert): (varint-delimited
+        DetectorSchemas, count), or None when the host encodes them -- the device declined the batch, the handle has no
+        encoder (a stand-in), or an ID does not fit the device's 64-bit integers."""
+        det = self.det
+        if not hasattr(det, "encode_alerts"):
+            return None
+        now = int(self.clock())
+        first_alert_id = self.start_id + self.n_alerts
+        if not (-(1 << 63) <= now < (1 << 63) and -(1 << 63) <= first_alert_id and first_alert_id + n_records < (1 << 63)
+                and 0 <= first_log_id and first_log_id + n_records < (1 << 64)):
+            return None
+        sig = (det, self.detector_id, self.method_type)
+        if self._alert_sig != sig:
+            combos = getattr(self, "combos", None) or []
+            names = self.logformat.header.names if self.logformat is not None else []
+            det.set_alert_format("1.0.0", self.detector_id, self.method_type, self._description(), self._alert_keys(), combos,
+                                 time_capture=names.index("Time") if "Time" in names else None)
+            self._alert_sig = sig
+        return det.encode_alerts(first_log_id, first_alert_id, now)
+
     def _description(self) -> str:
         return f"{self.detector_id} detects values not encountered in training as anomalies."
 
@@ -659,6 +708,13 @@ class B200NewValueComboDetector(B200NewValueDetector):
 
     def _description(self) -> str:
         return f"{self.detector_id} detects value combinations not encountered in training as anomalies."
+
+    def _alert_keys(self) -> List[Tuple[str, List[int]]]:
+        n = len(self.monitors)
+        by_key: Dict[str, List[int]] = {}
+        for c, members in enumerate(self.combos):
+            by_key.setdefault(self._combo_alert(members, [b""] * len(members))[0], []).append(n + c)
+        return sorted(by_key.items())
 
     def _combo_alert(self, members: List[int], values: List[bytes]) -> Tuple[str, str]:
         """("<scope> - (<label>, ...)", "Unknown value combination: ('v1', ...)") of one combination."""

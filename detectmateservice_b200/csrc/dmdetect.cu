@@ -20,6 +20,7 @@
 #include "dm_kernels_logs.cuh"
 #include "dm_kernels_format.cuh"
 #include "dm_kernels_lanes.cuh"
+#include "dm_kernels_alerts.cuh"
 #include "dm_format_host.h"
 
 static void (*g_nccl_destroy_hook)(void*) = nullptr;   // set once NCCL is loaded (dm_nccl_load)
@@ -110,6 +111,20 @@ struct dm_handle {
     uint32_t logs_chunks = 0;            // chunks they hold
     DmLogsHeader* d_lhdr = nullptr;
     DmLogsHeader* h_lhdr = nullptr;      // pinned
+    // DetectorSchema alerts on the device (dm_set_alert_format / dm_encode_alerts), allocated by dm_set_alert_format
+    const uint8_t* last_buf = nullptr;   // the last dm_process_lines batch as its kernels read it, and its scores
+    const float* last_scores = nullptr;
+    bool last_was_lines = false;         // the last batch came from dm_process_lines itself
+    DmAlertFmt* d_afmt = nullptr;
+    DmAlertHeader* d_ahdr = nullptr;
+    DmAlertHeader* h_ahdr = nullptr;     // pinned
+    void* d_alert = nullptr;             // rank (max_lines + 1), per anomalous record line / mask / offset / size, tile sums
+    uint8_t* d_aout = nullptr;           // the encoded alerts
+    uint64_t alert_cap = 0;              // bytes of d_aout
+    uint32_t alert_time_cap = DMA_NONE;  // log_format mode: the header capture named Time
+    DmFormat* h_fmt = nullptr;           // host copy of the last dm_set_format[_ex] format (the encoder's is built from it)
+    DmFormat* d_efmt = nullptr;          // the encoder's format: h_fmt keeping the Time capture too (dm_alert_efmt_build)
+    uint32_t efmt_slots = 1;
     // pipelined host path: two slots
     struct Slot {
         uint8_t* d_in = nullptr; uint8_t* d_flags = nullptr; float* d_scores = nullptr;
@@ -322,6 +337,8 @@ extern "C" int dm_destroy(dm_handle* h) {
     cudaFree(h->table.slots); cudaFree(h->table.novel); cudaFree(h->table.count);
     cudaFree(h->d_vals); cudaFree(h->d_masks); cudaFree(h->d_mons); cudaFree(h->d_fmt); cudaFree(h->d_norm);
     cudaFree(h->d_logs_text); cudaFree(h->d_logs); cudaFree(h->d_lhdr); cudaFreeHost(h->h_lhdr);
+    cudaFree(h->d_afmt); cudaFree(h->d_ahdr); cudaFreeHost(h->h_ahdr); cudaFree(h->d_alert); cudaFree(h->d_aout);
+    cudaFree(h->d_efmt); delete h->h_fmt;
     for (int k = 0; k < 2; ++k) {
         cudaFree(h->d_win[k]);
         if (h->ev_win_done[k]) cudaEventDestroy(h->ev_win_done[k]);
@@ -467,6 +484,9 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     }
     DM_CUDA(cudaGetLastError());
     if (!stream_kernel) h->dmx.chain_stream = nullptr;     // (a launch that is not the stream kernel's ends the overlap chain)
+    h->last_buf = d_buf;
+    h->last_scores = d_scores;
+    h->last_was_lines = true;
 
     const bool want_sync = host_out || n_lines_out || n_anomalies_out;
     if (!want_sync) return DM_OK;
@@ -511,6 +531,7 @@ extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blo
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
+    h->last_was_lines = false;
     if (n_values > h->vals_cap) {
         if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
         h->vals_cap = std::max<uint64_t>(2ull * n_values, 4096);
@@ -624,6 +645,8 @@ extern "C" int dm_set_combos(dm_handle* h, uint32_t n_combos, const uint32_t* me
 // log_format + templates (MatcherParser fused in front of the detector)
 // ---------------------------------------------------------------------------------------
 
+static int dm_alert_efmt_upload(dm_handle* h);
+
 extern "C" int dm_set_format(dm_handle* h, const char* log_format, const char* content_name, uint32_t n_templates,
                              const char* const* templates) {
     return dm_set_format_ex(h, log_format, content_name, n_templates, templates, 0);
@@ -654,10 +677,14 @@ extern "C" int dm_set_format_ex(dm_handle* h, const char* log_format, const char
         else {
             h->fmt_set = true;
             h->fmt_slots = f->max_slots;
+            delete h->h_fmt;
+            h->h_fmt = f;                                        // (kept: the alert encoder's format is built from it)
+            f = nullptr;
             h->fmt_norm = n_templates ? norm_flags : 0;             // (without templates there is nothing to normalise)
         }
     }
     delete f;
+    if (rc == DM_OK) rc = dm_alert_efmt_upload(h);
     return rc;
 }
 
@@ -715,6 +742,7 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
+    h->last_was_lines = false;
     if (2ull * n_records + 2 > 3ull * h->vals_cap + 1) {
         if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
         h->vals_cap = std::max<uint64_t>(2ull * n_records, 4096);
@@ -895,11 +923,13 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
         uint64_t n_lines = 0, n_anoms = 0;
         rc = dm_process_lines(h, h->d_logs_text, lh.total_bytes, 1, lh.n_train, nullptr, nullptr, 0, 0, &n_lines, &n_anoms, st);
         dm_break_chain(h, st);
+        h->last_was_lines = false;                            // (its anomaly list is rewritten to records below)
         if (rc != DM_OK) return rc;
         if (n_lines != lh.n_lines)
             return dm_fail(DM_ERR_STATE, "the line path found %llu records in %llu unwrapped texts", (unsigned long long)n_lines, (unsigned long long)lh.n_lines);
     } else {
         DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+        h->last_was_lines = false;
     }
     const int grid_s = (int)std::max<uint32_t>(1, std::min<uint32_t>(std::max<uint32_t>(tiles, h->anomaly_cap / DML_THREADS), (uint32_t)h->sm_count * 8));
     dm_k_logs_scatter<<<grid_s, DML_THREADS, 0, st>>>(a, h->d_flags, h->d_scores, d_rflags, d_rscores, h->d_anoms, h->anomaly_cap,
@@ -913,6 +943,144 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     if (n_records_out) *n_records_out = n_records;
     if (n_malformed_out) *n_malformed_out = n_records - lh.n_lines;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    return DM_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// DetectorSchema alerts of raw-line batches, encoded on the device (dm_kernels_alerts.cuh)
+// ---------------------------------------------------------------------------------------
+static uint64_t dm_alert_tiles(uint64_t n) { return (n + DMA_TILE - 1) / DMA_TILE; }
+
+// The encoder's copy of the log_format (when both the format and the alert format are set): the matcher's own, keeping
+// the Time capture as well.
+static int dm_alert_efmt_upload(dm_handle* h) {
+    if (!h->fmt_set || !h->h_fmt || !h->d_afmt) return DM_OK;
+    DmFormat* ef = new (std::nothrow) DmFormat;
+    if (!ef) return dm_fail(DM_ERR_ARG, "out of host memory");
+    dm_alert_efmt_build(*h->h_fmt, h->alert_time_cap, ef);
+    cudaError_t e = cudaSetDevice(h->device);
+    if (e == cudaSuccess && !h->d_efmt) e = cudaMalloc(&h->d_efmt, sizeof(DmFormat));
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->last_stream);
+    if (e == cudaSuccess) e = cudaMemcpy(h->d_efmt, ef, sizeof(DmFormat), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) h->efmt_slots = ef->max_slots;
+    delete ef;
+    if (e != cudaSuccess) return dm_fail(DM_ERR_CUDA, "encoder format: %s", cudaGetErrorString(e));
+    return DM_OK;
+}
+
+extern "C" int dm_set_alert_format(dm_handle* h, uint32_t n_strings, const uint8_t* strings, const uint32_t* string_lens,
+                                   const uint32_t* bits_off, const uint32_t* bits, uint32_t n_combos,
+                                   const uint32_t* combo_off, const uint32_t* combo_members, uint32_t time_capture,
+                                   uint64_t out_cap) {
+    if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
+    if (!string_lens || (!strings && n_strings)) return dm_fail(DM_ERR_ARG, "strings missing");
+    if (out_cap == 0) return dm_fail(DM_ERR_ARG, "out_cap must be positive");
+    DmAlertFmt* f = new (std::nothrow) DmAlertFmt;
+    if (!f) return dm_fail(DM_ERR_ARG, "out of host memory");
+    const char* why = dm_alert_fmt_build(h->h_keys, n_strings, strings, string_lens, bits_off, bits, n_combos, combo_off,
+                                         combo_members, time_capture, f);
+    if (why) { delete f; return dm_fail(DM_ERR_ARG, "dm_set_alert_format: %s", why); }
+    cudaError_t e = cudaSetDevice(h->device);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->last_stream);
+    if (e == cudaSuccess && !h->d_afmt) {
+        // everything the encoder needs, once: per record a rank, per anomaly-list entry a record's line, mask, offset and
+        // size, the scan's tile sums.  Allocated into locals and kept only when every allocation succeeded, so that a
+        // failed call leaves the handle without an encoder (and a later call allocates again).
+        const uint64_t lines = h->max_lines + 1, recs = (uint64_t)h->anomaly_cap + 1;
+        const uint64_t tiles = dm_alert_tiles(std::max(lines, recs)) + 1;
+        DmAlertFmt* d_afmt = nullptr;
+        DmAlertHeader *d_ahdr = nullptr, *h_ahdr = nullptr;
+        void* d_alert = nullptr;
+        e = cudaMalloc(&d_afmt, sizeof(DmAlertFmt));
+        if (e == cudaSuccess) e = cudaMalloc(&d_ahdr, sizeof(DmAlertHeader));
+        if (e == cudaSuccess) e = cudaHostAlloc(&h_ahdr, sizeof(DmAlertHeader), cudaHostAllocDefault);
+        if (e == cudaSuccess) e = cudaMalloc(&d_alert, 4 * lines + 8 + 8 * recs * 3 + 8 * tiles);
+        if (e == cudaSuccess) {
+            h->d_afmt = d_afmt; h->d_ahdr = d_ahdr; h->h_ahdr = h_ahdr; h->d_alert = d_alert;
+        } else {
+            cudaFree(d_afmt); cudaFree(d_ahdr); cudaFreeHost(h_ahdr); cudaFree(d_alert);
+        }
+    }
+    if (e == cudaSuccess && out_cap != h->alert_cap) {
+        cudaFree(h->d_aout);
+        h->d_aout = nullptr;
+        h->alert_cap = 0;
+        e = cudaMalloc(&h->d_aout, out_cap);
+        if (e == cudaSuccess) h->alert_cap = out_cap;
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(h->d_afmt, f, sizeof(DmAlertFmt), cudaMemcpyHostToDevice);
+    delete f;
+    if (e != cudaSuccess) return dm_fail(DM_ERR_CUDA, "dm_set_alert_format: %s", cudaGetErrorString(e));
+    h->alert_time_cap = time_capture < DM_FMT_MAX_CAPTURES ? time_capture : DMA_NONE;
+    return dm_alert_efmt_upload(h);
+}
+
+template <typename T>
+static void dm_alert_scan(T* d, uint64_t n, T* tile_sums, T* total, cudaStream_t st) {
+    const uint32_t tiles = (uint32_t)std::max<uint64_t>(1, dm_alert_tiles(n));
+    dm_k_alert_scan_tiles<T><<<tiles, DMA_THREADS, 0, st>>>(d, n, tile_sums);
+    dm_k_alert_scan_top<T><<<1, DMA_THREADS, 0, st>>>(tile_sums, tiles, total);
+    dm_k_alert_scan_apply<T><<<tiles, DMA_THREADS, 0, st>>>(d, n, tile_sums);
+}
+
+extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t first_alert_id, int64_t now, uint8_t* out,
+                                uint64_t out_cap, uint64_t* out_len, uint64_t* n_alerts, int* declined) {
+    if (!h || !out_len || !n_alerts || !declined) return dm_fail(DM_ERR_ARG, "NULL argument");
+    if (out_cap && !out) return dm_fail(DM_ERR_ARG, "out is NULL");
+    if (!h->d_afmt || !h->d_aout) return dm_fail(DM_ERR_STATE, "dm_set_alert_format has not been called");
+    if (!h->last_was_lines) return dm_fail(DM_ERR_STATE, "the last batch did not come from dm_process_lines");
+    *out_len = 0;
+    *n_alerts = 0;
+    *declined = 0;
+    int rc = dm_sync(h, nullptr, nullptr);
+    if (rc != DM_OK) return rc;
+    const uint32_t entries = std::min(h->h_hdr->anomaly_list_count, h->anomaly_cap);
+    const uint64_t n_lines = h->h_hdr->n_lines;
+    if (entries == 0 || n_lines == 0) return DM_OK;
+    cudaStream_t st = h->last_stream;
+    dm_break_chain(h, st);
+    const uint64_t lines = h->max_lines + 1, recs = (uint64_t)h->anomaly_cap + 1;
+    DmAlertArgs a;
+    a.fmt = h->d_afmt; a.buf = h->last_buf; a.nbytes = h->last_nbytes; a.scores = h->last_scores;
+    a.anoms = h->d_anoms; a.n_entries = entries; a.n_lines = n_lines;
+    a.rank = (uint32_t*)h->d_alert;
+    unsigned long long* w = (unsigned long long*)((uint8_t*)h->d_alert + ((4 * lines + 7) & ~7ull));
+    a.rec_off = w; a.size = w + recs;
+    unsigned long long* tile_sums = w + 2 * recs;
+    a.rec_line = (uint32_t*)(tile_sums + dm_alert_tiles(std::max(lines, recs)) + 1);
+    a.rec_mask = a.rec_line + recs;
+    a.ahdr = h->d_ahdr; a.first_log_id = first_log_id; a.first_alert_id = first_alert_id; a.now = now;
+    a.out = h->d_aout; a.out_cap = std::min(out_cap, h->alert_cap);
+    a.efmt = h->d_efmt; a.nbuf = h->d_norm;
+    // log_format mode: the size and write passes re-run the matcher (one thread per record, DM_FMTL_THREADS per CTA)
+    const bool fmt = h->fmt_set, norm = h->fmt_norm != 0;
+    if (fmt && !h->d_efmt) return dm_fail(DM_ERR_STATE, "no log_format for the alert encoder");
+    const size_t fsmem = (size_t)2 * h->efmt_slots * DM_FMTL_THREADS * sizeof(uint2);
+    const int fgrid = (int)std::max<uint32_t>(1, std::min<uint32_t>((entries + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS, (uint32_t)h->sm_count * 32));
+    const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>((entries + DMA_THREADS - 1) / DMA_THREADS, (uint32_t)h->sm_count * 8));
+    DM_CUDA(cudaMemsetAsync(h->d_ahdr, 0, sizeof(DmAlertHeader), st));
+    DM_CUDA(cudaMemsetAsync(a.rank, 0, n_lines * 4, st));
+    DM_CUDA(cudaMemsetAsync(a.rec_mask, 0, (uint64_t)entries * 4, st));
+    dm_k_alert_mark<<<grid, DMA_THREADS, 0, st>>>(a);
+    dm_alert_scan<uint32_t>(a.rank, n_lines, (uint32_t*)tile_sums, &h->d_ahdr->n_alerts, st);
+    dm_k_alert_gather<<<grid, DMA_THREADS, 0, st>>>(a);
+    if (!fmt) dm_k_alert_size<<<grid, DMA_THREADS, 0, st>>>(a);
+    else if (norm) dm_k_alert_format<true, false><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
+    else dm_k_alert_format<false, false><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
+    dm_alert_scan<unsigned long long>(a.size, entries, tile_sums, &h->d_ahdr->total, st);
+    if (!fmt) dm_k_alert_write<<<grid, DMA_THREADS, 0, st>>>(a);
+    else if (norm) dm_k_alert_format<true, true><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
+    else dm_k_alert_format<false, true><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
+    h->launches += 10;
+    DM_CUDA(cudaGetLastError());
+    DM_CUDA(cudaMemcpyAsync(h->h_ahdr, h->d_ahdr, sizeof(DmAlertHeader), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
+    const DmAlertHeader ah = *h->h_ahdr;
+    *n_alerts = ah.n_alerts;
+    *out_len = ah.total;
+    if (ah.declined || ah.total > a.out_cap) { *declined = 1; return DM_OK; }
+    if (ah.total) DM_CUDA(cudaMemcpyAsync(out, h->d_aout, ah.total, cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
     return DM_OK;
 }
 
@@ -961,6 +1129,7 @@ extern "C" int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t n
     DM_CUDA(cudaEventRecord(sl.ev_in, h->st_in));
     cudaStream_t st = h->stream;                       // ONE compute stream: submission order = processing order
     h->last_stream = st;
+    h->last_was_lines = false;
     DM_CUDA(cudaStreamWaitEvent(st, sl.ev_in, 0));
     if (nbytes == 0) DM_CUDA(cudaMemsetAsync(sl.d_hdr, 0, sizeof(DmBatchHeader), st));
     const int launched = dmx_launch(&h->dmx, sl.d_in, nbytes, n_train_lines, h->table, sl.d_flags, sl.d_scores, h->max_lines, sl.d_anoms,
@@ -1125,6 +1294,7 @@ extern "C" int dm_import_known(dm_handle* h, const uint64_t* keys, uint64_t n) {
     DM_CUDA(cudaMemcpy(d_tmp, keys, n * sizeof(unsigned long long), cudaMemcpyHostToDevice));
     DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), h->last_stream));
     dm_break_chain(h, h->last_stream);
+    h->last_was_lines = false;
     dm_k_insert_keys<<<std::max(1, (int)std::min<uint64_t>((n + 255) / 256, 1024)), 256, 0, h->last_stream>>>(h->table, d_tmp, n, &h->d_hdr->error);
     DM_CUDA(cudaGetLastError());
     int rc = dm_sync(h, nullptr, nullptr);

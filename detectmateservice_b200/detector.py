@@ -268,6 +268,46 @@ class DeviceDetector:
         k = n_rec.value
         return flags[:k], scores[:k], int(n_bad.value)
 
+    # ------------------------------------------------------------------ DetectorSchema alerts on the device
+    def set_alert_format(self, version: str, detector_id: str, detector_type: str, description: str,
+                         alert_keys: Sequence[Tuple[str, Sequence[int]]], combos: Sequence[Sequence[int]] = (),
+                         capacity: int = 0, time_capture: Optional[int] = None) -> None:
+        """What encode_alerts() writes besides the record's own values (dm_set_alert_format): the constant strings, the
+        alertsObtain keys in output order, each with the mask bits that supply it in config order (bit k < n monitors =
+        monitor k, bit n + c = combination c, whose monitors `combos[c]` lists), the capacity of the output buffer in
+        bytes (0: a quarter of max_batch_bytes, at least 1 MiB) and, in log_format mode, the index of the header capture
+        that holds the record's Time (None: none).  Allocates the buffers once."""
+        strs = [s.encode("utf-8") for s in (version, detector_id, detector_type, description)]
+        strs += [k.encode("utf-8") for k, _bits in alert_keys]
+        lens = (C.c_uint32 * len(strs))(*[len(s) for s in strs])
+        off, flat = [0], []
+        for _k, bits in alert_keys:
+            flat.extend(int(b) for b in bits)
+            off.append(len(flat))
+        c_off, c_mem = [0], []
+        for members in combos:
+            c_mem.extend(int(i) for i in members)
+            c_off.append(len(c_mem))
+        cap = int(capacity) or max(1 << 20, self.max_batch_bytes // 4)
+        _lib.check(self._lib.dm_set_alert_format(
+            self._h, len(strs), b"".join(strs), lens, (C.c_uint32 * len(off))(*off), (C.c_uint32 * max(1, len(flat)))(*flat),
+            len(combos), (C.c_uint32 * len(c_off))(*c_off), (C.c_uint32 * max(1, len(c_mem)))(*c_mem),
+            0xFFFFFFFF if time_capture is None else int(time_capture), cap))
+        if getattr(self, "_pin_alerts", None) is None or self._pin_alerts.numel() != cap:
+            import torch
+            self._pin_alerts = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
+
+    def encode_alerts(self, first_log_id: int, first_alert_id: int, now: int) -> Optional[Tuple[bytes, int]]:
+        """The varint-delimited DetectorSchemas of the last process_lines() batch (dm_encode_alerts) and their count, or
+        None when the device declines the batch (the caller then encodes it on the host)."""
+        out_len, n, declined = C.c_uint64(), C.c_uint64(), C.c_int()
+        buf = self._pin_alerts
+        _lib.check(self._lib.dm_encode_alerts(self._h, int(first_log_id), int(first_alert_id), int(now), buf.data_ptr(),
+                                              buf.numel(), C.byref(out_len), C.byref(n), C.byref(declined)))
+        if declined.value:
+            return None
+        return bytes(buf.numpy()[:out_len.value]), int(n.value)
+
     def sync(self) -> Tuple[int, int]:
         n_lines = C.c_uint64()
         n_anom = C.c_uint64()

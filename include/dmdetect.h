@@ -244,6 +244,40 @@ int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delim
                     uint8_t* flags_out, float* scores_out, uint64_t out_cap,
                     uint64_t* n_records_out, uint64_t* n_malformed_out, uint64_t* n_anomalies_out);
 
+/* DetectorSchema alerts of a raw-line batch, encoded on the device (rule R-alert, DESIGN.md): the bytes the component's
+ * host encoder writes for the same batch (component.py _line_alerts / _format_alerts / _detector_schema,
+ * wire.encode_detector_schema), in key=value mode and in log_format mode (dm_set_format[_ex]).
+ * dm_set_alert_format fixes what does not change from call to call and allocates, once, the device buffers, of which
+ * the output buffer holds out_cap bytes:
+ *   strings / string_lens : n_strings strings, concatenated: __version__, detectorID, detectorType, description, then
+ *                           the alert keys (alertsObtain keys) in output order, i.e. sorted by their UTF-8 bytes;
+ *   bits_off / bits       : alert key j is supplied by the mask bits bits[bits_off[j], bits_off[j + 1]) in config
+ *                           order; of those set in a record's mask the last one wins.  A bit below n_keys is monitor
+ *                           k, worded "Unknown value: '<v>'"; bit n_keys + c is combination c, whose monitors are
+ *                           combo_members[combo_off[c], combo_off[c + 1]) ("Unknown value combination: ('<v1>', ...)").
+ *                           Monitor k's value: key=value mode, the first true field of key k of dm_create (R-tok
+ *                           L2-L6); log_format mode, its header capture verbatim or its template variable (under
+ *                           R-norm a slice of the normalised Content);
+ *   time_capture          : log_format mode: the header capture whose text is the record's Time, 0xFFFFFFFF = none
+ *                           (key=value mode always takes msg=audit(<Time>...), R-tok L7).
+ * dm_encode_alerts encodes the last batch of dm_process_lines (whichever kernel ran it) into `out`: one varint-length-
+ * delimited DetectorSchema per anomalous record, in record order; alertID = first_alert_id + j (signed), logIDs =
+ * [first_log_id + record index], detectionTimestamp = receivedTimestamp = now, extractedTimestamps = [int(float(Time))],
+ * or now when the record has no Time or its Time is no float literal.  *n_alerts = anomalous records, *out_len = bytes.
+ * *declined = 1 when the device cannot give the host's bytes: a Time string it cannot convert with certainty (outside
+ * [0-9]{1,10}(\.[0-9]{0,6})? yet made only of bytes a float literal may hold), or an output larger than min(out_cap,
+ * the out_cap of dm_set_alert_format) (*out_len then tells how large); the caller then encodes that batch on the host.
+ * Synchronous; ends the overlap chain of dm_process_lines.  The encoder reads the batch's message, its scores and its
+ * anomaly list, which the next overlapped call rewrites; so a device-resident caller must leave that call's `buf` --
+ * and its `scores_out`, when it passed a device scores buffer -- unchanged until dm_encode_alerts returns, and must not
+ * enqueue another dm_process_lines on the handle in between.  DM_ERR_STATE when the last batch came from another entry
+ * point (dm_process_logs, dm_process_records, dm_process_values, the pipelined path). */
+int dm_set_alert_format(dm_handle* h, uint32_t n_strings, const uint8_t* strings, const uint32_t* string_lens,
+                        const uint32_t* bits_off, const uint32_t* bits, uint32_t n_combos, const uint32_t* combo_off,
+                        const uint32_t* combo_members, uint32_t time_capture, uint64_t out_cap);
+int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t first_alert_id, int64_t now, uint8_t* out,
+                     uint64_t out_cap, uint64_t* out_len, uint64_t* n_alerts, int* declined);
+
 /* Pipelined host path (two slots): dm_submit_lines enqueues, without waiting, the copy of a
  * HOST message (pinned memory gives real overlap) to the device, the kernels and the copy
  * of the batch header back; dm_collect waits for that slot, copies the slot's flags and
