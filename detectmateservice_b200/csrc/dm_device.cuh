@@ -202,6 +202,29 @@ struct DmDetectArgs {
     const void* combos;               // lanes / format kernel with combinations: const DmMonitors* (else NULL)
 };
 
+// The thread-per-record kernels' arguments for a message K_A has indexed into line_start (line_lo / line_hi are set
+// per launch).
+static inline DmDetectArgs dm_detect_args(const uint8_t* buf, uint64_t nbytes, const uint32_t* line_start, DmBatchHeader* hdr,
+                                          const DmKeys* keys, DmTable table, uint8_t* flags, float* scores, uint64_t out_cap,
+                                          dm_anomaly_t* anomalies, uint32_t anomaly_cap, unsigned long long* stats,
+                                          const void* combos) {
+    DmDetectArgs a{};
+    a.buf = buf; a.nbytes = nbytes; a.line_start = line_start; a.hdr_in = hdr; a.hdr = hdr; a.keys = keys; a.table = table;
+    a.flags = flags; a.scores = scores; a.out_cap = out_cap; a.anomalies = anomalies; a.anomaly_cap = anomaly_cap;
+    a.stats = stats; a.combos = combos;
+    return a;
+}
+
+// Their grid.  The number of records is only known on the device: the grid is sized for the most the message can hold
+// (one per byte pair, at most max_lines), capped at max_grid CTAs (the kernels stride); CTAs past the last record leave
+// after one compare.
+static inline unsigned dm_detect_grid(uint64_t nbytes, uint64_t max_lines, unsigned threads, uint64_t max_grid) {
+    const uint64_t max_recs = nbytes / 2 + 1 < max_lines ? nbytes / 2 + 1 : max_lines;
+    const uint64_t want = (max_recs + threads - 1) / threads;
+    const uint64_t grid = want < max_grid ? want : max_grid;
+    return (unsigned)(grid > 1 ? grid : 1);
+}
+
 // ---------------------------------------------------------------------------------------
 // byte-level helpers shared by the kernels (R-tok, DESIGN.md section 2)
 // ---------------------------------------------------------------------------------------

@@ -393,3 +393,17 @@ __global__ void __launch_bounds__(DM_FMTL_THREADS) dm_k_format_lanes(DmDetectArg
             atomicAdd(&a.stats[8 + threadIdx.x], (unsigned long long)s_unk[threadIdx.x]);
     }
 }
+
+// R-norm runs when normalisation is configured and there are templates to run on the normalised Content.
+static inline bool dm_format_norm(const DmFormat& f) { return f.norm_flags != 0 && f.n_chains > 1; }
+
+// The instantiation a launch runs.
+typedef void (*DmFormatLanesKernel)(DmDetectArgs, const DmFormat*, uint8_t*);
+static inline DmFormatLanesKernel dm_format_lanes_kernel(bool train, bool norm, bool combo) {
+    if (train) {
+        if (norm) return combo ? dm_k_format_lanes<true, true, true> : dm_k_format_lanes<true, true, false>;
+        return combo ? dm_k_format_lanes<true, false, true> : dm_k_format_lanes<true, false, false>;
+    }
+    if (norm) return combo ? dm_k_format_lanes<false, true, true> : dm_k_format_lanes<false, true, false>;
+    return combo ? dm_k_format_lanes<false, false, true> : dm_k_format_lanes<false, false, false>;
+}

@@ -230,6 +230,23 @@ __global__ void __launch_bounds__(DMR_A_THREADS) dm_k_rowindex(DmRowsArgs a) {
     }
 }
 
+// K_A's arguments for one message, writing the record index to line_start.  The look-back tag *epoch advances when
+// the message has rows (else nothing is launched).  The fields dm_k_rowindex does not read stay zero.
+static inline DmRowsArgs dm_rows_args(const uint8_t* buf, uint64_t nbytes, uint32_t* row_prefix, unsigned long long* tile_state,
+                                      uint32_t* epoch, uint32_t* line_start, uint8_t* flags, float* scores, uint64_t out_cap,
+                                      DmBatchHeader* hdr, unsigned long long* stats, uint64_t n_train_lines, uint64_t max_lines) {
+    DmRowsArgs a{};
+    a.buf = buf; a.nbytes = nbytes;
+    a.n_rows = (uint32_t)((nbytes + DMR_ROW - 1) / DMR_ROW);
+    a.n_tiles = (a.n_rows + DMR_TILE_ROWS - 1) / DMR_TILE_ROWS;
+    a.row_prefix = row_prefix; a.tile_state = tile_state;
+    if (a.n_rows) *epoch = (*epoch % 0x3FFFFFFEu) + 1u;
+    a.epoch = *epoch;
+    a.line_start = line_start; a.flags = flags; a.scores = scores; a.out_cap = out_cap;
+    a.hdr = hdr; a.stats = stats; a.n_train_lines = n_train_lines; a.max_lines = max_lines;
+    return a;
+}
+
 #ifndef DM_EMU
 // ---------------------------------------------------------------------------------------
 // host side
@@ -237,9 +254,7 @@ __global__ void __launch_bounds__(DMR_A_THREADS) dm_k_rowindex(DmRowsArgs a) {
 struct DmRowsScratch {
     uint32_t* d_row_prefix = nullptr;
     unsigned long long* d_tile_state = nullptr;
-    unsigned long long* d_row_ctr = nullptr;
     uint64_t max_rows = 0, max_tiles = 0;
-    unsigned long long ctr_base = 0;
     uint32_t epoch = 0;
     // K_A reads the message before it waits for its predecessor (programmatic dependent launch); a caller may have
     // produced that message with a kernel of its own on the same stream, so K_A is launched as an ordinary kernel
@@ -253,16 +268,13 @@ static inline int dm_rows_scratch_create(DmRowsScratch* s, uint64_t max_batch_by
     if (cudaMalloc(&s->d_row_prefix, s->max_rows * sizeof(uint32_t)) != cudaSuccess) return DM_ERR_CUDA;
     if (cudaMalloc(&s->d_tile_state, s->max_tiles * sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
     if (cudaMemset(s->d_tile_state, 0, s->max_tiles * sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMalloc(&s->d_row_ctr, sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMemset(s->d_row_ctr, 0, sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
     return DM_OK;
 }
 
 static inline void dm_rows_scratch_destroy(DmRowsScratch* s) {
     cudaFree(s->d_row_prefix);
     cudaFree(s->d_tile_state);
-    cudaFree(s->d_row_ctr);
-    s->d_row_prefix = nullptr; s->d_tile_state = nullptr; s->d_row_ctr = nullptr;
+    s->d_row_prefix = nullptr; s->d_tile_state = nullptr;
 }
 
 // <<<>>> with the programmatic-stream-serialization attribute (see dm_pdl_wait)

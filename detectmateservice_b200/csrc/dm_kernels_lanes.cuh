@@ -179,6 +179,13 @@ __global__ void __launch_bounds__(DM_LANES_THREADS) dm_k_lanes(DmDetectArgs a) {
     }
 }
 
+// The instantiation a launch runs.
+typedef void (*DmLanesKernel)(DmDetectArgs);
+static inline DmLanesKernel dm_lanes_kernel(bool train, bool combo) {
+    if (train) return combo ? dm_k_lanes<true, true> : dm_k_lanes<true, false>;
+    return combo ? dm_k_lanes<false, true> : dm_k_lanes<false, false>;
+}
+
 #ifndef DM_EMU
 // K_A (row index + record index) then one thread per record.  Returns the number of launches.
 static inline int dm_lanes_launch(DmRowsScratch* s, uint32_t* d_line_start, const uint8_t* d_buf, uint64_t nbytes,
@@ -187,47 +194,28 @@ static inline int dm_lanes_launch(DmRowsScratch* s, uint32_t* d_line_start, cons
                                   DmBatchHeader* d_hdr, unsigned long long* d_stats, uint64_t max_lines, int sm_count,
                                   const void* d_combos, uint32_t n_keys,
                                   cudaStream_t st, void (*mark)(void*, cudaStream_t, int), void* mark_ctx) {
-    const uint32_t n_rows = (uint32_t)((nbytes + DMR_ROW - 1) / DMR_ROW);
-    if (n_rows == 0) return 0;
-    if (n_rows > s->max_rows) return DM_ERR_CAPACITY;
-    DmRowsArgs ra;
-    ra.buf = d_buf; ra.nbytes = nbytes; ra.n_rows = n_rows;
-    ra.n_tiles = (n_rows + DMR_TILE_ROWS - 1) / DMR_TILE_ROWS;
-    ra.row_prefix = s->d_row_prefix; ra.tile_state = s->d_tile_state;
-    s->epoch = (s->epoch % 0x3FFFFFFEu) + 1u;
-    ra.epoch = s->epoch;
-    ra.keys = d_keys; ra.table = table; ra.flags = d_flags; ra.scores = d_scores; ra.out_cap = out_cap;
-    ra.anomalies = d_anoms; ra.anomaly_cap = anomaly_cap; ra.hdr = d_hdr; ra.stats = d_stats;
-    ra.row_ctr = s->d_row_ctr; ra.n_train_lines = n_train_lines; ra.max_lines = max_lines;
-    ra.line_lo = 0; ra.line_hi = ~0ull; ra.ctr_base = s->ctr_base; ra.aux_counts = nullptr;
-    ra.line_start = d_line_start; ra.group = DMR_GROUP; ra.static_rows = 0; ra.timeline = nullptr;
+    if ((nbytes + DMR_ROW - 1) / DMR_ROW > s->max_rows) return DM_ERR_CAPACITY;
+    const DmRowsArgs ra = dm_rows_args(d_buf, nbytes, s->d_row_prefix, s->d_tile_state, &s->epoch, d_line_start, d_flags,
+                                       d_scores, out_cap, d_hdr, d_stats, n_train_lines, max_lines);
+    if (ra.n_rows == 0) return 0;
     int launched = 0;
     dm_launch_pdl(dm_k_rowindex, ra.n_tiles, DMR_A_THREADS, st, s->pdl, ra);
     ++launched;
-    DmDetectArgs a;
-    a.buf = d_buf; a.line_start = d_line_start; a.hdr_in = d_hdr; a.hdr = d_hdr; a.keys = d_keys; a.table = table;
-    a.flags = d_flags; a.scores = d_scores; a.out_cap = out_cap; a.anomalies = d_anoms; a.anomaly_cap = anomaly_cap;
-    a.stats = d_stats; a.nbytes = nbytes;
-    // the number of records is only known on the device: size the grid for one record per
-    // byte pair at most and let the kernel stride; unused CTAs exit after one compare
-    const uint64_t max_recs = std::min<uint64_t>(nbytes / 2 + 1, max_lines);
-    const uint64_t want = (max_recs + DM_LANES_THREADS - 1) / DM_LANES_THREADS;
-    const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)sm_count * 32));
+    DmDetectArgs a = dm_detect_args(d_buf, nbytes, d_line_start, d_hdr, d_keys, table, d_flags, d_scores, out_cap, d_anoms,
+                                    anomaly_cap, d_stats, d_combos);
+    const unsigned grid = dm_detect_grid(nbytes, max_lines, DM_LANES_THREADS, (uint64_t)sm_count * 32);
     // (the record kernels themselves are launched normally: their records sit in the first CTAs of
     // a worst-case grid, and an early launch into whatever slots K_A leaves free places those
     // CTAs unevenly -- measured 2x slower; the next step's K_A still overlaps their tail)
-    a.combos = d_combos;
     const size_t smem = d_combos ? (size_t)n_keys * DM_LANES_THREADS * sizeof(unsigned long long) : 0;
     if (n_train_lines > 0) {
         a.line_lo = 0; a.line_hi = n_train_lines;
-        if (d_combos) dm_launch_pdl_smem(dm_k_lanes<true, true>, (unsigned)grid, DM_LANES_THREADS, smem, st, false, a);
-        else dm_launch_pdl_smem(dm_k_lanes<true, false>, (unsigned)grid, DM_LANES_THREADS, 0, st, false, a);
+        dm_launch_pdl_smem(dm_lanes_kernel(true, d_combos != nullptr), grid, DM_LANES_THREADS, smem, st, false, a);
         ++launched;
     }
     a.line_lo = n_train_lines; a.line_hi = ~0ull;
     if (mark) mark(mark_ctx, st, 0);
-    if (d_combos) dm_launch_pdl_smem(dm_k_lanes<false, true>, (unsigned)grid, DM_LANES_THREADS, smem, st, false, a);
-    else dm_launch_pdl_smem(dm_k_lanes<false, false>, (unsigned)grid, DM_LANES_THREADS, 0, st, false, a);
+    dm_launch_pdl_smem(dm_lanes_kernel(false, d_combos != nullptr), grid, DM_LANES_THREADS, smem, st, false, a);
     if (mark) mark(mark_ctx, st, 1);
     ++launched;
     if (cudaGetLastError() != cudaSuccess) return DM_ERR_CUDA;

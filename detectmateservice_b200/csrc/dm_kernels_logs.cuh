@@ -57,6 +57,17 @@ struct DmLogsArgs {
     DmLogsHeader* lhdr;
 };
 
+// The walk's plan for n_records records on at most max_ctas CTAs, each a contiguous chunk of whole DML_THREADS-record
+// tiles: *per_cta = records per chunk; returns the number of chunks (the walk's grid).
+static inline uint32_t dm_logs_plan(uint32_t n_records, uint32_t max_ctas, uint32_t* per_cta) {
+    const uint32_t tiles = (n_records + DML_THREADS - 1) / DML_THREADS;
+    const uint32_t want = tiles < max_ctas ? tiles : max_ctas;
+    const uint32_t ctas = want > 1 ? want : 1;
+    const uint32_t tiles_per_cta = (tiles + ctas - 1) / ctas;
+    *per_cta = (tiles_per_cta > 1 ? tiles_per_cta : 1) * DML_THREADS;
+    return (n_records + *per_cta - 1) / *per_cta;
+}
+
 // Walks one LogSchema record [pos, end).  False where protobuf's runtime refuses the record, and for a group; else
 // [tp, tp + tl) is the last `log` field (tl = 0 when there is none).  A field 1-5 under another wire type is an
 // unknown field to protobuf and skipped; an unknown LEN field is not checked for UTF-8.

@@ -1287,6 +1287,19 @@ __global__ void __launch_bounds__(256) dm_k_bound(const uint8_t* __restrict__ bu
     }
 }
 
+// Geometry of a launch over a.n_rows rows on at most max_grid CTAs: every warp gets the same number of contiguous rows.
+// Sets a.rows_per_warp / rows_per_cta / ctas_per_grp; returns the grid.
+static inline unsigned dmx_geometry(DmxArgs& a, uint64_t max_grid) {
+    const unsigned long long warps_max = max_grid * DMX_WARPS;
+    const uint32_t rpw = (uint32_t)((a.n_rows + warps_max - 1) / warps_max);
+    const unsigned long long warps = (a.n_rows + rpw - 1) / rpw;
+    const unsigned grid = (unsigned)((warps + DMX_WARPS - 1) / DMX_WARPS);
+    a.rows_per_warp = rpw;
+    a.rows_per_cta = rpw * DMX_WARPS;
+    a.ctas_per_grp = (grid + DMX_THREADS - 1) / DMX_THREADS;
+    return grid;
+}
+
 #ifndef DM_EMU
 // ---------------------------------------------------------------------------------------
 // host side
@@ -1403,14 +1416,7 @@ static inline int dmx_launch(DmxScratch* s, const uint8_t* d_buf, uint64_t nbyte
         chained = (hint & 0xFFFFFFFFull) != 0 && (hint >> 32) * 4ull >= (hint & 0xFFFFFFFFull);
     }
     s->last_chained = chained;
-    // geometry: every warp gets the same number of contiguous rows
-    const unsigned long long warps_max = (unsigned long long)s->max_grid * DMX_WARPS;
-    const uint32_t rpw = (uint32_t)((n_rows + warps_max - 1) / warps_max);
-    const unsigned long long warps = (n_rows + rpw - 1) / rpw;
-    const unsigned grid = (unsigned)((warps + DMX_WARPS - 1) / DMX_WARPS);
-    a.rows_per_warp = rpw;
-    a.rows_per_cta = rpw * DMX_WARPS;
-    a.ctas_per_grp = (grid + DMX_THREADS - 1) / DMX_THREADS;
+    const unsigned grid = dmx_geometry(a, (uint64_t)s->max_grid);
     s->last_grid = grid;
     int launched = 0;
     auto bind = [&]() {

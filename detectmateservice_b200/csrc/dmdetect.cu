@@ -22,6 +22,7 @@
 #include "dm_kernels_lanes.cuh"
 #include "dm_kernels_alerts.cuh"
 #include "dm_format_host.h"
+#include "dm_host.h"
 
 static void (*g_nccl_destroy_hook)(void*) = nullptr;   // set once NCCL is loaded (dm_nccl_load)
 
@@ -95,7 +96,7 @@ struct dm_handle {
     DmMonitors h_mons;             // host copy (dm_set_monitors + dm_set_combos)
     DmFormat* d_fmt = nullptr;     // log_format + templates (dm_set_format)
     uint8_t* d_norm = nullptr;     // R-norm: the message's normalised Content text (dm_set_format_ex with flags)
-    uint32_t fmt_norm = 0;
+    bool fmt_norm = false;         // R-norm runs (dm_format_norm)
     void* nccl_comm[2] = {nullptr, nullptr};   // own NCCL communicators (dm_nccl_init): windows alternate between them
     uint32_t nccl_n = 0, nccl_rank = 0, nccl_world = 1;
     unsigned long long* d_win[2] = {nullptr, nullptr};   // window exchange buffers of dm_window_allreduce
@@ -412,12 +413,10 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     const bool host_out = !out_on_device && (flags_out || scores_out);
     uint8_t* d_flags = (out_on_device && flags_out) ? flags_out : h->d_flags;
     float* d_scores = (out_on_device && scores_out) ? scores_out : h->d_scores;
-    const uint64_t dev_cap = out_on_device ? ((flags_out || scores_out) ? out_cap_lines : h->max_lines) : h->max_lines;
     // when only one of the two outputs is a caller device buffer the other stays internal
     const uint64_t cap_flags = (out_on_device && flags_out) ? out_cap_lines : h->max_lines;
     const uint64_t cap_scores = (out_on_device && scores_out) ? out_cap_lines : h->max_lines;
     const uint64_t out_cap = std::min(cap_flags, cap_scores);
-    (void)dev_cap;
 
     bool stream_kernel = false;
     // (the stream kernel and K_A write the per-batch header themselves)
@@ -426,44 +425,27 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
 
     if (h->fmt_set) {
         // log_format / template mode: K_A writes the record index, then one THREAD per record
-        const uint32_t n_rows = (uint32_t)((nbytes + DMR_ROW - 1) / DMR_ROW);
-        if (n_rows > h->rows.max_rows) return dm_fail(DM_ERR_CAPACITY, "message too large for the row index");
-        if (n_rows > 0) {
-            DmRowsArgs ra;
-            ra.buf = d_buf; ra.nbytes = nbytes; ra.n_rows = n_rows;
-            ra.n_tiles = (n_rows + DMR_TILE_ROWS - 1) / DMR_TILE_ROWS;
-            ra.row_prefix = h->rows.d_row_prefix; ra.tile_state = h->rows.d_tile_state;
-            h->rows.epoch = (h->rows.epoch % 0x3FFFFFFEu) + 1u;
-            ra.epoch = h->rows.epoch;
-            ra.keys = h->d_keys; ra.table = h->table; ra.flags = d_flags; ra.scores = d_scores; ra.out_cap = out_cap;
-            ra.anomalies = h->d_anoms; ra.anomaly_cap = h->anomaly_cap; ra.hdr = h->d_hdr; ra.stats = h->d_stats;
-            ra.row_ctr = h->rows.d_row_ctr; ra.n_train_lines = n_train_lines; ra.max_lines = h->max_lines;
-            ra.line_lo = 0; ra.line_hi = ~0ull; ra.ctr_base = h->rows.ctr_base; ra.aux_counts = nullptr;
-            ra.line_start = h->d_line_start; ra.group = DMR_GROUP; ra.static_rows = 0; ra.timeline = nullptr;
+        if ((nbytes + DMR_ROW - 1) / DMR_ROW > h->rows.max_rows) return dm_fail(DM_ERR_CAPACITY, "message too large for the row index");
+        const DmRowsArgs ra = dm_rows_args(d_buf, nbytes, h->rows.d_row_prefix, h->rows.d_tile_state, &h->rows.epoch, h->d_line_start,
+                                           d_flags, d_scores, out_cap, h->d_hdr, h->d_stats, n_train_lines, h->max_lines);
+        if (ra.n_rows > 0) {
             dm_launch_pdl(dm_k_rowindex, ra.n_tiles, DMR_A_THREADS, st, h->rows.pdl, ra);
-            DmDetectArgs a;
-            a.buf = d_buf; a.line_start = h->d_line_start; a.hdr_in = h->d_hdr; a.hdr = h->d_hdr;
-            a.keys = h->d_keys; a.table = h->table; a.flags = d_flags; a.scores = d_scores; a.out_cap = out_cap;
-            a.anomalies = h->d_anoms; a.anomaly_cap = h->anomaly_cap; a.stats = h->d_stats; a.nbytes = nbytes;
             // combination monitors: the COMBO instantiations re-hash their members from the captures the lanes keep
             const bool combos = h->mons_set && h->h_mons.n_combos > 0;
-            a.combos = combos ? (const void*)h->d_mons : nullptr;
-            const uint64_t max_recs = std::min<uint64_t>(nbytes / 2 + 1, h->max_lines);
-            const uint64_t want = (max_recs + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS;
-            const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * 32));
+            DmDetectArgs a = dm_detect_args(d_buf, nbytes, h->d_line_start, h->d_hdr, h->d_keys, h->table, d_flags, d_scores, out_cap,
+                                            h->d_anoms, h->anomaly_cap, h->d_stats, combos ? (const void*)h->d_mons : nullptr);
+            const unsigned grid = dm_detect_grid(nbytes, h->max_lines, DM_FMTL_THREADS, (uint64_t)h->sm_count * 32);
             const size_t smem = (size_t)2 * h->fmt_slots * DM_FMTL_THREADS * sizeof(uint2);
-            const bool norm = h->fmt_norm != 0;
+            const bool norm = h->fmt_norm;
             if (n_train_lines > 0) {
                 a.line_lo = 0; a.line_hi = n_train_lines;
-                auto k = combos ? (norm ? dm_k_format_lanes<true, true, true> : dm_k_format_lanes<true, false, true>)
-                                : (norm ? dm_k_format_lanes<true, true, false> : dm_k_format_lanes<true, false, false>);
-                dm_launch_pdl_smem(k, (unsigned)grid, DM_FMTL_THREADS, smem, st, false, a, (const DmFormat*)h->d_fmt, h->d_norm);
+                dm_launch_pdl_smem(dm_format_lanes_kernel(true, norm, combos), grid, DM_FMTL_THREADS, smem, st, false, a,
+                                   (const DmFormat*)h->d_fmt, h->d_norm);
             }
             a.line_lo = n_train_lines; a.line_hi = ~0ull;
             dm_prof_mark(h, st, 0);
-            auto k = combos ? (norm ? dm_k_format_lanes<false, true, true> : dm_k_format_lanes<false, false, true>)
-                            : (norm ? dm_k_format_lanes<false, true, false> : dm_k_format_lanes<false, false, false>);
-            dm_launch_pdl_smem(k, (unsigned)grid, DM_FMTL_THREADS, smem, st, false, a, (const DmFormat*)h->d_fmt, h->d_norm);
+            dm_launch_pdl_smem(dm_format_lanes_kernel(false, norm, combos), grid, DM_FMTL_THREADS, smem, st, false, a,
+                               (const DmFormat*)h->d_fmt, h->d_norm);
             dm_prof_mark(h, st, 1);
             h->launches += 2 + (n_train_lines > 0 ? 1 : 0);
         }
@@ -513,6 +495,16 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
 // ---------------------------------------------------------------------------------------
 // record mode
 // ---------------------------------------------------------------------------------------
+// Adds what a synchronous record call counts on the host (dm_stats_add_records) to the handle's statistics.
+static int dm_records_stats(dm_handle* h, uint64_t n_records, uint64_t trained, uint64_t scored, uint64_t nbytes) {
+    unsigned long long cur[6];
+    DM_CUDA(cudaMemcpy(cur, h->d_stats, sizeof(cur), cudaMemcpyDeviceToHost));
+    dm_stats_add_records(cur, n_records, trained, scored, nbytes);
+    DM_CUDA(cudaMemcpy(h->d_stats, cur, 3 * sizeof(cur[0]), cudaMemcpyHostToDevice));
+    DM_CUDA(cudaMemcpy(h->d_stats + 5, &cur[5], sizeof(cur[5]), cudaMemcpyHostToDevice));
+    return DM_OK;
+}
+
 extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blob_bytes, const uint32_t* offsets,
                                  const uint32_t* fields, const uint32_t* record_of, uint32_t n_values,
                                  uint32_t n_records, uint32_t n_train_records, uint64_t record_bytes,
@@ -570,18 +562,11 @@ extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blo
     if (masks_out && n_records) DM_CUDA(cudaMemcpyAsync(masks_out, h->d_masks, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
     // statistics that do not need the device: record and byte counts
-    {
-        const unsigned long long tr = std::min<uint32_t>(n_train_records, n_records);
-        unsigned long long add[6] = {n_records, tr, n_records - tr, 0, 0, record_bytes};
-        unsigned long long cur[6];
-        DM_CUDA(cudaMemcpy(cur, h->d_stats, sizeof(cur), cudaMemcpyDeviceToHost));
-        cur[0] += add[0]; cur[1] += add[1]; cur[2] += add[2]; cur[5] += add[5];
-        unsigned long long upd[3] = {cur[0], cur[1], cur[2]};
-        DM_CUDA(cudaMemcpy(h->d_stats, upd, sizeof(upd), cudaMemcpyHostToDevice));
-        DM_CUDA(cudaMemcpy(h->d_stats + 5, &cur[5], sizeof(unsigned long long), cudaMemcpyHostToDevice));
-    }
+    const uint32_t tr = std::min<uint32_t>(n_train_records, n_records);
+    int rc = dm_records_stats(h, n_records, tr, n_records - tr, record_bytes);
+    if (rc != DM_OK) return rc;
     h->h_hdr->n_lines = n_records;
-    int rc = dm_check_device_errors(h);
+    rc = dm_check_device_errors(h);
     if (rc != DM_OK) return rc;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
     return DM_OK;
@@ -680,7 +665,7 @@ extern "C" int dm_set_format_ex(dm_handle* h, const char* log_format, const char
             delete h->h_fmt;
             h->h_fmt = f;                                        // (kept: the alert encoder's format is built from it)
             f = nullptr;
-            h->fmt_norm = n_templates ? norm_flags : 0;             // (without templates there is nothing to normalise)
+            h->fmt_norm = dm_format_norm(*h->h_fmt);
         }
     }
     delete f;
@@ -709,6 +694,13 @@ extern "C" int dm_debug_rows_timeline(dm_handle* h, unsigned long long* out, uin
     return dm_fail(DM_ERR_STATE, "create the handle with DM_STREAM_TIMELINE=1");
 }
 
+// The error of a framing split (dm_frame_split).
+static int dm_frame_fail(const DmFrames& f) {
+    if (f.error == DM_FRAME_TRUNCATED) return dm_fail(DM_ERR_ARG, "truncated length prefix at byte %llu", (unsigned long long)f.at);
+    return dm_fail(DM_ERR_ARG, "record of %llu bytes at byte %llu runs past the end of the message", (unsigned long long)f.rec_len,
+                   (unsigned long long)f.at);
+}
+
 extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nbytes, uint32_t n_train_records,
                                   uint8_t* flags_out, float* scores_out, uint32_t* masks_out, uint64_t out_cap,
                                   uint64_t* n_records_out, uint64_t* n_anomalies_out) {
@@ -716,24 +708,10 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     if (!h->mons_set) return dm_fail(DM_ERR_STATE, "dm_set_monitors has not been called");
     if (nbytes && !buf) return dm_fail(DM_ERR_ARG, "buf is NULL");
     if (nbytes > h->max_batch_bytes) return dm_fail(DM_ERR_CAPACITY, "message of %llu bytes exceeds max_batch_bytes=%llu", (unsigned long long)nbytes, (unsigned long long)h->max_batch_bytes);
-    // framing: varint length, payload, varint length, payload ...
-    std::vector<uint32_t> off, len;
-    uint64_t pos = 0;
-    while (pos < nbytes) {
-        uint64_t l = 0;
-        int shift = 0;
-        for (;;) {
-            if (pos >= nbytes || shift > 63) return dm_fail(DM_ERR_ARG, "truncated length prefix at byte %llu", (unsigned long long)pos);
-            const uint8_t b = buf[pos++];
-            l |= (uint64_t)(b & 0x7F) << shift;
-            if (!(b & 0x80)) break;
-            shift += 7;
-        }
-        if (l > nbytes - pos) return dm_fail(DM_ERR_ARG, "record of %llu bytes at byte %llu runs past the end of the message", (unsigned long long)l, (unsigned long long)pos);
-        off.push_back((uint32_t)pos);
-        len.push_back((uint32_t)l);
-        pos += l;
-    }
+    const DmFrames fr = dm_frame_split(buf, nbytes);
+    if (fr.error) return dm_frame_fail(fr);
+    const std::vector<uint32_t>& off = fr.off;
+    const std::vector<uint32_t>& len = fr.len;
     const uint32_t n_records = (uint32_t)off.size();
     if (n_records > h->max_lines) return dm_fail(DM_ERR_CAPACITY, "%u records exceed max_lines=%llu", n_records, (unsigned long long)h->max_lines);
     if ((flags_out || scores_out || masks_out) && n_records > out_cap)
@@ -786,18 +764,12 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     if (masks_out && n_records) DM_CUDA(cudaMemcpyAsync(masks_out, h->d_masks, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
     if (n_records && n_train_records > 0) DM_CUDA(cudaMemcpyAsync(bound, d_bound, sizeof(bound), cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
-    {
-        // train_lines: the records trained; detect_lines: the records from the bound on (malformed ones included)
-        const unsigned long long tr = bound[1], first_scored = n_train_records > 0 ? bound[0] : 0;
-        unsigned long long cur[6];
-        DM_CUDA(cudaMemcpy(cur, h->d_stats, sizeof(cur), cudaMemcpyDeviceToHost));
-        unsigned long long upd[3] = {cur[0] + n_records, cur[1] + tr, cur[2] + (n_records - first_scored)};
-        const unsigned long long nb = cur[5] + nbytes;
-        DM_CUDA(cudaMemcpy(h->d_stats, upd, sizeof(upd), cudaMemcpyHostToDevice));
-        DM_CUDA(cudaMemcpy(h->d_stats + 5, &nb, sizeof(nb), cudaMemcpyHostToDevice));
-    }
+    // train_lines: the records trained; detect_lines: the records from the bound on (malformed ones included)
+    const uint64_t first_scored = n_train_records > 0 ? bound[0] : 0;
+    int rc = dm_records_stats(h, n_records, bound[1], n_records - first_scored, nbytes);
+    if (rc != DM_OK) return rc;
     h->h_hdr->n_lines = n_records;
-    int rc = dm_check_device_errors(h);
+    rc = dm_check_device_errors(h);
     if (rc != DM_OK) return rc;
     if (n_records_out) *n_records_out = n_records;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
@@ -859,27 +831,16 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     if (nbytes && !buf) return dm_fail(DM_ERR_ARG, "buf is NULL");
     if (nbytes > h->max_batch_bytes) return dm_fail(DM_ERR_CAPACITY, "message of %llu bytes exceeds max_batch_bytes=%llu", (unsigned long long)nbytes, (unsigned long long)h->max_batch_bytes);
     // framing: one bare record, or varint length, payload, varint length, payload ...
-    std::vector<uint32_t> off, len;
-    if (!delimited) {
-        off.push_back(0);
-        len.push_back((uint32_t)nbytes);
+    DmFrames fr;
+    if (delimited) {
+        fr = dm_frame_split(buf, nbytes);
+        if (fr.error) return dm_frame_fail(fr);
+    } else {
+        fr.off.push_back(0);
+        fr.len.push_back((uint32_t)nbytes);
     }
-    uint64_t pos = 0;
-    while (delimited && pos < nbytes) {
-        uint64_t l = 0;
-        int shift = 0;
-        for (;;) {
-            if (pos >= nbytes || shift > 63) return dm_fail(DM_ERR_ARG, "truncated length prefix at byte %llu", (unsigned long long)pos);
-            const uint8_t b = buf[pos++];
-            l |= (uint64_t)(b & 0x7F) << shift;
-            if (!(b & 0x80)) break;
-            shift += 7;
-        }
-        if (l > nbytes - pos) return dm_fail(DM_ERR_ARG, "record of %llu bytes at byte %llu runs past the end of the message", (unsigned long long)l, (unsigned long long)pos);
-        off.push_back((uint32_t)pos);
-        len.push_back((uint32_t)l);
-        pos += l;
-    }
+    const std::vector<uint32_t>& off = fr.off;
+    const std::vector<uint32_t>& len = fr.len;
     const uint32_t n_records = (uint32_t)off.size();
     if (n_records > h->max_lines) return dm_fail(DM_ERR_CAPACITY, "%u records exceed max_lines=%llu", n_records, (unsigned long long)h->max_lines);
     if ((flags_out || scores_out) && n_records > out_cap)
@@ -888,11 +849,10 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
-    // walk grid: at most 4 CTAs per SM, each a contiguous chunk of whole DML_THREADS-record tiles
+    // walk grid: at most 4 CTAs per SM
+    uint32_t per_cta;
+    const uint32_t n_chunks = dm_logs_plan(n_records, (uint32_t)h->sm_count * 4, &per_cta);
     const uint32_t tiles = (n_records + DML_THREADS - 1) / DML_THREADS;
-    const uint32_t want = std::max<uint32_t>(1, std::min<uint32_t>(tiles, (uint32_t)h->sm_count * 4));
-    const uint32_t per_cta = std::max<uint32_t>(1, (tiles + want - 1) / want) * DML_THREADS;
-    const uint32_t n_chunks = (n_records + per_cta - 1) / per_cta;
     int rc = dm_logs_reserve(h, n_records, n_chunks);
     if (rc != DM_OK) return rc;
     float* d_rscores;
@@ -1053,7 +1013,7 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     a.out = h->d_aout; a.out_cap = std::min(out_cap, h->alert_cap);
     a.efmt = h->d_efmt; a.nbuf = h->d_norm;
     // log_format mode: the size and write passes re-run the matcher (one thread per record, DM_FMTL_THREADS per CTA)
-    const bool fmt = h->fmt_set, norm = h->fmt_norm != 0;
+    const bool fmt = h->fmt_set, norm = h->fmt_norm;
     if (fmt && !h->d_efmt) return dm_fail(DM_ERR_STATE, "no log_format for the alert encoder");
     const size_t fsmem = (size_t)2 * h->efmt_slots * DM_FMTL_THREADS * sizeof(uint2);
     const int fgrid = (int)std::max<uint32_t>(1, std::min<uint32_t>((entries + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS, (uint32_t)h->sm_count * 32));
@@ -1168,18 +1128,15 @@ extern "C" int dm_collect(dm_handle* h, uint32_t slot, const uint8_t** flags_out
     return DM_OK;
 }
 
+// Reads the anomaly list of a batch (total entries written, at most anomaly_cap of them kept) and merges it
+// (dm_anomalies_merge): *n_out = the records, the first cap of them go to out.
 static int dm_fetch_anomalies(dm_handle* h, const dm_anomaly_t* d_list, uint32_t total, dm_anomaly_t* out, uint32_t cap, uint32_t* n_out) {
     const uint32_t have = std::min(total, h->anomaly_cap);
     *n_out = 0;
     if (have == 0) return DM_OK;
     std::vector<dm_anomaly_t> tmp(have);
     DM_CUDA(cudaMemcpy(tmp.data(), d_list, (uint64_t)have * sizeof(dm_anomaly_t), cudaMemcpyDeviceToHost));
-    std::sort(tmp.begin(), tmp.end(), [](const dm_anomaly_t& a, const dm_anomaly_t& b) { return a.line < b.line; });
-    uint32_t m = 0;
-    for (uint32_t i = 0; i < have; ++i) {
-        if (m && tmp[m - 1].line == tmp[i].line) { tmp[m - 1].mask |= tmp[i].mask; continue; }
-        tmp[m++] = tmp[i];
-    }
+    const uint32_t m = dm_anomalies_merge(tmp.data(), have);
     *n_out = m;
     if (out && cap) memcpy(out, tmp.data(), (uint64_t)std::min(m, cap) * sizeof(dm_anomaly_t));
     return DM_OK;
@@ -1215,20 +1172,8 @@ extern "C" int dm_get_anomalies(dm_handle* h, dm_anomaly_t* out, uint32_t cap, u
     if (rc != DM_OK) return rc;
     const uint32_t total = h->h_hdr->anomaly_list_count;
     *n_out = std::min<uint64_t>(total, h->h_hdr->n_anomalies ? h->h_hdr->n_anomalies : total);
-    const uint32_t have = std::min(total, h->anomaly_cap);
-    if (!out || cap == 0 || have == 0) return DM_OK;
-    std::vector<dm_anomaly_t> tmp(have);
-    DM_CUDA(cudaMemcpy(tmp.data(), h->d_anoms, (uint64_t)have * sizeof(dm_anomaly_t), cudaMemcpyDeviceToHost));
-    std::sort(tmp.begin(), tmp.end(), [](const dm_anomaly_t& a, const dm_anomaly_t& b) { return a.line < b.line; });
-    // the fused kernel appends one entry per unknown field: merge the entries of a record
-    uint32_t m = 0;
-    for (uint32_t i = 0; i < have; ++i) {
-        if (m && tmp[m - 1].line == tmp[i].line) { tmp[m - 1].mask |= tmp[i].mask; continue; }
-        tmp[m++] = tmp[i];
-    }
-    *n_out = m;
-    memcpy(out, tmp.data(), (uint64_t)std::min(m, cap) * sizeof(dm_anomaly_t));
-    return DM_OK;
+    if (!out || cap == 0 || std::min(total, h->anomaly_cap) == 0) return DM_OK;
+    return dm_fetch_anomalies(h, h->d_anoms, total, out, cap, n_out);
 }
 
 static void dm_words_to_stats(const unsigned long long* w, dm_stats_t* out) {

@@ -1,7 +1,6 @@
 """NewValueComboDetector (SURVEY.md section 8f-4): tuples of field values.  Oracle semantics (R-combo,
 oracle/nvcd.py -- parity unpinned, defined by us), the kernel source on the CPU emulator,
 the component's alert wording against the oracle, and (GPU tier) the real library."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -104,31 +103,19 @@ def test_emu_combo_kernel():
     recs = make_records(1000)
     want_f, want_s, want_m, _, orc = oracle_run(recs)
     assert sum(want_f) > 40 and any(s > 1 for s in want_s)
-    lib = C.CDLL(emu_harness.build())
     det = emu_harness.EmuDetector([b"\x01m%d" % i for i in range(len(orc.monitors))], table_log2=12)
-    arr = _monitor_array(orc.monitors)
-    off, flat = [0], []
-    for m in orc.combos:
-        flat += m
-        off.append(len(flat))
-    lib.emu_set_combos.argtypes = [C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32]
-    lib.emu_set_combos(len(orc.combos), (C.c_uint32 * len(off))(*off), (C.c_uint32 * len(flat))(*flat), (1 << len(orc.monitors)) - 1)
-    lib.emu_process_records.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint64, C.c_uint32,
-                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    det.set_monitors(_monitor_array(orc.monitors), len(orc.monitors))
+    det.set_combos(orc.combos, (1 << len(orc.monitors)) - 1)
     got_f, got_s, got_m, seen = [], [], [], 0
-    try:
-        for lo in range(0, len(recs), 300):
-            batch = wire.frame_delimited([wire.encode_parser_schema(r) for r in recs[lo:lo + 300]])
-            n_train = max(0, min(300, 400 - seen))
-            f = np.full(300, 9, np.uint8); s = np.full(300, -1, np.float32); m = np.zeros(300, np.uint32)
-            n_rec, n_an = C.c_uint64(), C.c_uint64()
-            assert lib.emu_process_records(det.h, arr, len(orc.monitors), batch, len(batch), n_train, f.ctypes.data,
-                                           s.ctypes.data, m.ctypes.data, 300, C.byref(n_rec), C.byref(n_an)) == 0
-            k = n_rec.value
-            seen += k
-            got_f += f[:k].tolist(); got_s += s[:k].tolist(); got_m += m[:k].tolist()
-    finally:
-        lib.emu_set_combos(0, (C.c_uint32 * 1)(0), (C.c_uint32 * 1)(0), 0)
+    for lo in range(0, len(recs), 300):
+        batch = wire.frame_delimited([wire.encode_parser_schema(r) for r in recs[lo:lo + 300]])
+        n_train = max(0, min(300, 400 - seen))
+        f = np.full(300, 9, np.uint8); s = np.full(300, -1, np.float32); m = np.zeros(300, np.uint32)
+        rc, k, _ = det.process_records(batch, n_train, f, s, m, 300)
+        assert rc == 0
+        seen += k
+        got_f += f[:k].tolist(); got_s += s[:k].tolist(); got_m += m[:k].tolist()
+    det.close()
     assert got_f == want_f and got_s == want_s and got_m == want_m
 
 
@@ -293,23 +280,15 @@ def test_emu_raw_combo_kernel():
     assert sum(want_f) > 60 and any(s >= 2 for s in want_s)
     keys = [m.pos.encode() for m in orc.monitors]
     det = emu_harness.EmuDetector(keys, table_log2=12, variant="lanes")
-    off, flat = [0], []
-    for m in orc.combos:
-        flat += m
-        off.append(len(flat))
-    lib = det.lib
-    lib.emu_set_combos.argtypes = [C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32]
-    lib.emu_set_combos(len(orc.combos), (C.c_uint32 * len(off))(*off), (C.c_uint32 * len(flat))(*flat), (1 << len(keys)) - 1)
-    try:
-        buf = b"\n".join(lines) + b"\n"
-        cut = buf.index(b"\n", len(buf) // 2) + 1
-        f1, s1 = det.process_lines(buf[:cut], 1500)
-        an = det.anomalies()
-        n1 = len(f1)
-        f2, s2 = det.process_lines(buf[cut:], max(0, 1500 - n1))
-        an2 = det.anomalies()
-    finally:
-        lib.emu_set_combos(0, (C.c_uint32 * 1)(0), (C.c_uint32 * 1)(0), 0)
+    det.set_combos(orc.combos, (1 << len(keys)) - 1)
+    buf = b"\n".join(lines) + b"\n"
+    cut = buf.index(b"\n", len(buf) // 2) + 1
+    f1, s1 = det.process_lines(buf[:cut], 1500)
+    an = det.anomalies()
+    n1 = len(f1)
+    f2, s2 = det.process_lines(buf[cut:], max(0, 1500 - n1))
+    an2 = det.anomalies()
+    det.close()
     assert f1.tolist() + f2.tolist() == want_f and s1.tolist() + s2.tolist() == want_s
     got_m = {a[0]: a[1] for a in an}
     got_m.update({a[0] + n1: a[1] for a in an2})

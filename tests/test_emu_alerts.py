@@ -5,7 +5,6 @@ component's host encoder writes it for the same batch."""
 import ctypes as C
 import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
@@ -16,99 +15,44 @@ from detectmateservice_b200.synth import MONITORED_KEYS, AuditSynth
 NOW = 1773848383
 
 
-def _emu_lib():
-    import emu_harness
-    src = os.path.join(emu_harness.EMU, "emu_alerts.cpp")
-    so = os.path.join(emu_harness.EMU, "_build", "libemu_alerts.so")
-    deps = [src, os.path.join(emu_harness.EMU, "emu_tile.cpp"), os.path.join(emu_harness.EMU, "emu_format_combo.cpp"), os.path.join(emu_harness.EMU, "cuda_emu.h")] + [
-        os.path.join(emu_harness.CSRC, f) for f in os.listdir(emu_harness.CSRC)] + [
-        os.path.join(emu_harness.ROOT, "include", "dmdetect.h")]
-    if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        # (-Bsymbolic: the library binds to its own emulator runtime, whatever else the process has loaded)
-        subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-DDM_EMU", "-I" + emu_harness.EMU, "-I" + emu_harness.CSRC,
-                               "-shared", "-fPIC", "-pthread", "-Wl,-Bsymbolic", "-o", so, src])
-    lib = C.CDLL(so)
-    fn = [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
-          C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
-    for name in ("emu_process_stream", "emu_process_stream_chain", "emu_process_lanes", "emu_process_format_combo"):
-        getattr(lib, name).argtypes = fn
-    lib.emu_create.restype = C.c_void_p
-    lib.emu_create.argtypes = [C.c_uint32, C.c_char_p, C.POINTER(C.c_uint32), C.c_uint32, C.c_uint64, C.c_uint64]
-    lib.emu_destroy.argtypes = [C.c_void_p]
-    lib.emu_set_combos.argtypes = [C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32]
-    lib.emu_get_anomalies.restype = C.c_uint32
-    lib.emu_get_anomalies.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
-    lib.emu_set_alert_format.restype = C.c_char_p
-    lib.emu_set_alert_format.argtypes = [C.c_void_p, C.c_uint32, C.c_char_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
-                                         C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
-                                         C.c_uint32]
-    lib.emu_set_format.restype = C.c_char_p
-    lib.emu_set_format.argtypes = [C.c_void_p, C.c_uint32, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_char_p),
-                                   C.c_uint32]
-    lib.emu_encode_alerts.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_int64, C.c_int64,
-                                      C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
-    lib.emu_utf8_replace.restype = C.c_uint32
-    lib.emu_utf8_replace.argtypes = [C.c_char_p, C.c_uint32, C.c_void_p]
-    lib.emu_alert_time.argtypes = [C.c_char_p, C.c_uint32, C.c_longlong, C.POINTER(C.c_longlong)]
-    return lib
-
-
 @pytest.fixture(scope="module")
 def lib():
-    return _emu_lib()
-
-
-class _Anomaly(C.Structure):
-    _fields_ = [("line", C.c_uint32), ("mask", C.c_uint32), ("offset", C.c_uint64)]
+    import emu_harness
+    return emu_harness.lib()
 
 
 class EmuDevice:
     """Stands in for DeviceDetector: detection and the alert encoder on the CPU emulator (tests only)."""
 
     def __init__(self, lib, keys, variant="stream", combos=(), capacity=1 << 20, comp=None):
+        import emu_harness
         self.lib, self.variant, self.capacity = lib, variant, capacity
+        self.det = emu_harness.EmuDetector([bytes(k) for k in keys], table_log2=14, variant=variant)
+        self.h = self.det.h
         if variant == "format":                                      # the component's log_format, templates, R-norm
             from test_format_combos import _monitor_array
             lf = comp.logformat
-            ts = [t if isinstance(t, bytes) else t.encode() for t in lf.template_sources]
-            err = lib.emu_set_format(_monitor_array(comp.monitors), len(comp.monitors), lf.source.encode(),
-                                     lf.content_name.encode(), len(ts), (C.c_char_p * max(1, len(ts)))(*ts), lf.flags)
-            assert err is None, err
-        self.keys = [bytes(k) for k in keys]
-        lens = (C.c_uint32 * max(1, len(self.keys)))(*[len(k) for k in self.keys])
-        self.h = lib.emu_create(len(self.keys), b"".join(self.keys), lens, 14, 64, 1 << 20)
-        off, flat = [0], []
-        for members in combos:
-            flat.extend(members)
-            off.append(len(flat))
-        lib.emu_set_combos(len(combos), (C.c_uint32 * len(off))(*off), (C.c_uint32 * max(1, len(flat)))(*flat),
-                           (1 << len(self.keys)) - 1 if combos else 0)
+            self.det.set_monitors(_monitor_array(comp.monitors), len(comp.monitors))
+            self.det.set_format(lf.source, lf.template_sources, lf.flags, lf.content_name.encode())
+        self.det.set_combos(combos, (1 << len(keys)) - 1 if combos else 0)
         self.last_n_anomalies = 0
         self.encoded = self.declined = 0
 
     def close(self):
-        if self.h:
-            self.lib.emu_destroy(self.h)
-            self.h = None
+        self.det.close()
+        self.h = None
 
     def process_lines(self, buf, n_train_lines=0, copy=True):
         self._msg = bytes(buf)
         cap = self._msg.count(b"\n") + 2
         flags, scores = np.zeros(cap, np.uint8), np.zeros(cap, np.float32)
-        n, na, err = C.c_uint64(), C.c_uint64(), C.c_uint32()
-        fn = {"stream": self.lib.emu_process_stream, "chain": self.lib.emu_process_stream_chain,
-              "lanes": self.lib.emu_process_lanes, "format": self.lib.emu_process_format_combo}[self.variant]
-        assert fn(self.h, self._msg, len(self._msg), n_train_lines, flags.ctypes.data, scores.ctypes.data, cap,
-                  C.byref(n), C.byref(na), C.byref(err)) == 0 and err.value == 0
+        f, s = self.det.process_lines(self._msg, n_train_lines, out=(flags, scores))
         self._scores = scores
-        self.last_n_anomalies = na.value
-        return flags[:n.value], scores[:n.value]
+        self.last_n_anomalies = self.det.last_n_anomalies
+        return f, s
 
     def anomalies(self):
-        arr = (_Anomaly * 65536)()
-        k = self.lib.emu_get_anomalies(self.h, arr, 65536)
-        return [(arr[i].line, arr[i].mask, arr[i].offset) for i in range(k)]
+        return self.det.anomalies()
 
     def set_alert_format(self, version, detector_id, detector_type, description, alert_keys, combos=(), capacity=0,
                          time_capture=None):

@@ -6,7 +6,6 @@ in between.  The messages here are built to hold each of those rows, a row made 
 32-byte lane holds five '=' or more, and a dense partial last row; quoted look-alikes and repeated keys make the
 re-check (one by one, and chained) decide many candidates.
 """
-import ctypes
 import random
 
 import numpy as np
@@ -106,7 +105,7 @@ def test_emu_lookup_rounds(variant):
     f = _check(det, o, _message(2), 0)
     assert 0 < f.sum() < f.size
     _check(det, o, _message(3, tail=False), 0)
-    lib = ctypes.CDLL(emu_harness.build())
+    lib = det.lib
     lib.emu_stream_ctas(40)                                             # a few rows per warp
     try:
         _check(det, o, _message(4), 0)

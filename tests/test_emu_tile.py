@@ -148,10 +148,7 @@ def test_emu_synthetic_and_split():
     assert st["unknown_per_key"] == [o.unknown_count(i) for i in range(len(keys))]
     assert st["lines"] == 4000 + 2500 and st["train_lines"] == 1500
     if VARIANT != "lanes":
-        import ctypes as C
-        lib = C.CDLL(emu_harness.build())
-        lib.emu_stream_hint.restype = C.c_uint64
-        hint = lib.emu_stream_hint()
+        hint = det.lib.emu_stream_hint()
         assert (hint >> 32) * 4 < (hint & 0xFFFFFFFF), hint              # rare anomalies: the host stays with the one-by-one re-check
     det.close()
 
@@ -181,8 +178,8 @@ def test_emu_lookalikes_and_duplicates(seed):
     det = EmuDetector(keys)
     _check(det, o, lookalike_lines(seed, 200), 80)
     import ctypes as C
-    lib = C.CDLL(emu_harness.build())
-    st = (C.c_ulonglong * 8)()
+    lib = det.lib
+    st = (C.c_uint64 * 8)()
     lib.emu_chain_stats(st, 1)
     f, _ = _check(det, o, lookalike_lines(seed + 50, 300), 0)
     assert 20 < f.sum() < f.size
@@ -200,7 +197,6 @@ def test_emu_lookalikes_and_duplicates(seed):
                 lib.emu_stream_ctas(3)
         _check(det, o, lookalike_lines(seed + 50, 300), 0)
         # what the host's choice of instantiation rests on: most batches of this message held a candidate
-        lib.emu_stream_hint.restype = C.c_uint64
         hint = lib.emu_stream_hint()
         rows, slow = hint & 0xFFFFFFFF, hint >> 32
         assert rows > 100 and slow * 4 >= rows, (rows, slow)
@@ -220,11 +216,6 @@ def test_emu_everything_unknown():
     det.close()
 
 
-def _emu_lib():
-    import ctypes as C
-    return C.CDLL(emu_harness.build())
-
-
 def test_emu_byte_position_sweep():
     """'=' on every residue mod 32 and at the 1 KiB row edges, the first '=' at bytes 1-4, values ending before, at and
     behind the 32-byte window and the 64 bytes behind a row, quoted spaces around the window's end, messages ending
@@ -241,7 +232,7 @@ def test_emu_byte_position_sweep():
         alerts += int(f.sum())
     assert alerts > len(msgs) // 2
     if VARIANT != "lanes":
-        lib = _emu_lib()
+        lib = det.lib
         lib.emu_stream_ctas(40)
         try:
             for m in msgs:

@@ -135,88 +135,24 @@ def _monitor_array(mons):
     return arr
 
 
-def _set_combos(lib, combos, member_only):
-    off, flat = [0], []
-    for m in combos:
-        flat += m
-        off.append(len(flat))
-    lib.emu_set_combos.argtypes = [C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32]
-    lib.emu_set_combos(len(combos), (C.c_uint32 * len(off))(*off), (C.c_uint32 * max(1, len(flat)))(*flat), member_only)
-
-
-def _clear_combos(lib):
-    lib.emu_set_combos(0, (C.c_uint32 * 1)(0), (C.c_uint32 * 1)(0), 0)
-
-
-def build_combo_emu():
-    """g++ tests/emu/emu_format_combo.cpp (the emulator of emu_tile.cpp plus the COMBO launches of the format kernel)
-    -> tests/emu/_build/libemu_format_combo.so, rebuilt when a source is newer."""
-    import subprocess
-    import emu_harness
-    src = os.path.join(emu_harness.EMU, "emu_format_combo.cpp")
-    so = os.path.join(emu_harness.EMU, "_build", "libemu_format_combo.so")
-    deps = [src, os.path.join(emu_harness.EMU, "emu_tile.cpp"), os.path.join(emu_harness.EMU, "cuda_emu.h"),
-            os.path.join(emu_harness.ROOT, "include", "dmdetect.h")] + [
-        os.path.join(emu_harness.CSRC, f) for f in os.listdir(emu_harness.CSRC)]
-    if os.path.exists(so) and all(os.path.getmtime(d) <= os.path.getmtime(so) for d in deps):
-        return so
-    os.makedirs(os.path.dirname(so), exist_ok=True)
-    # (-Bsymbolic: the library binds to its own emulator runtime, whatever else the process has loaded)
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-DDM_EMU", "-I" + emu_harness.EMU, "-I" + emu_harness.CSRC,
-                           "-shared", "-fPIC", "-pthread", "-Wl,-Bsymbolic", "-o", so, src])
-    return so
-
-
-def combo_emu_detector(n_keys, table_log2=14, max_lines=1 << 20):
-    """An emu_harness.EmuDetector whose handle lives in libemu_format_combo.so (anomalies / export_known / close work
-    as usual; the key names only matter to key=value records)."""
-    import emu_harness
-    det = emu_harness.EmuDetector.__new__(emu_harness.EmuDetector)
-    L = det.lib = C.CDLL(build_combo_emu())
-    L.emu_create.restype = C.c_void_p
-    L.emu_create.argtypes = [C.c_uint32, C.c_char_p, C.POINTER(C.c_uint32), C.c_uint32, C.c_uint64, C.c_uint64]
-    L.emu_destroy.argtypes = [C.c_void_p]
-    L.emu_get_anomalies.restype = C.c_uint32
-    L.emu_get_anomalies.argtypes = [C.c_void_p, C.POINTER(emu_harness.Anomaly), C.c_uint32]
-    L.emu_export_known.restype = C.c_uint64
-    L.emu_export_known.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.c_uint64]
-    det.variant = "format"
-    det.keys = [b"\x01m%d" % i for i in range(n_keys)]
-    lens = (C.c_uint32 * max(1, n_keys))(*[len(k) for k in det.keys])
-    det.h = L.emu_create(n_keys, b"".join(det.keys), lens, table_log2, (4 << 20) // emu_harness.TILE_BYTES + 2, max_lines)
-    det.max_lines = max_lines
-    return det
-
-
 class EmuFormatCombo:
-    """The kernel source on the emulator: emu_set_format + emu_set_combos + emu_process_format_combo.  The
-    combinations are set for each call and cleared in a finally."""
+    """The kernel source on the emulator: emu_set_monitors + emu_set_format + emu_set_combos + emu_process_format."""
 
     def __init__(self, mons, combos, member_only, log_format, templates=(), flags=0):
+        import emu_harness
         self.mons, self.combos, self.member_only = mons, combos, member_only
-        self.det = combo_emu_detector(len(mons))
-        L = self.lib = self.det.lib
-        L.emu_set_format.restype = C.c_char_p
-        L.emu_set_format.argtypes = [C.c_void_p, C.c_uint32, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_char_p), C.c_uint32]
-        L.emu_process_format_combo.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
-                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
-        L.emu_get_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
-        ts = [t if isinstance(t, bytes) else t.encode() for t in templates]
-        fmt = log_format if isinstance(log_format, bytes) else log_format.encode()
-        err = L.emu_set_format(_monitor_array(mons), len(mons), fmt, b"Content", len(ts), (C.c_char_p * max(1, len(ts)))(*ts), flags)
-        if err:
-            raise ValueError(err.decode())
+        self.det = emu_harness.EmuDetector([b"\x01m%d" % i for i in range(len(mons))], table_log2=14)
+        self.lib = self.det.lib
+        self.det.set_monitors(_monitor_array(mons), len(mons))
+        self.det.set_format(log_format, templates, flags)
+        self.det.set_combos(combos, member_only)
 
     def process(self, buf, n_train):
         cap = buf.count(b"\n") + 2
         f = np.full(cap, 9, np.uint8); s = np.full(cap, -1, np.float32)
         n, na, err = C.c_uint64(), C.c_uint64(), C.c_uint32()
-        _set_combos(self.lib, self.combos, self.member_only)
-        try:
-            rc = self.lib.emu_process_format_combo(self.det.h, buf, len(buf), n_train, f.ctypes.data, s.ctypes.data, cap,
-                                             C.byref(n), C.byref(na), C.byref(err))
-        finally:
-            _clear_combos(self.lib)
+        rc = self.lib.emu_process_format(self.det.h, buf, len(buf), n_train, f.ctypes.data, s.ctypes.data, cap,
+                                         C.byref(n), C.byref(na), C.byref(err))
         assert rc == 0 and err.value == 0
         k = n.value
         assert na.value == int(f[:k].sum())
@@ -461,20 +397,14 @@ def test_emu_key_equivalence_with_parser_schema(golden_dir):
         assert all(r is not None for r in recs)
         batch = wire.frame_delimited([wire.encode_parser_schema(_schema_record(r)) for r in recs])
         det = emu_harness.EmuDetector([b"\x01m%d" % i for i in range(len(mons))], table_log2=14)
-        L = det.lib
-        L.emu_process_records.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint64, C.c_uint32,
-                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        det.set_monitors(_monitor_array(mons), len(mons))
+        det.set_combos(combos, member_only)
         f = np.zeros(n, np.uint8); s = np.zeros(n, np.float32); m = np.zeros(n, np.uint32)
-        nr, na = C.c_uint64(), C.c_uint64()
-        _set_combos(L, combos, member_only)
-        try:
-            assert L.emu_process_records(det.h, _monitor_array(mons), len(mons), batch, len(batch), n, f.ctypes.data,
-                                         s.ctypes.data, m.ctypes.data, n, C.byref(nr), C.byref(na)) == 0
-        finally:
-            _clear_combos(L)
+        rc, nr, _ = det.process_records(batch, n, f, s, m, n)
+        assert rc == 0
         k_rec = sorted(det.export_known())
         det.close()
-        assert nr.value == n and len(k_fmt) > 40 and k_fmt == k_rec, norm
+        assert nr == n and len(k_fmt) > 40 and k_fmt == k_rec, norm
 
 
 # ------------------------------------------------------------------------------------------ component, device faked

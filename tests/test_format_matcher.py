@@ -160,19 +160,10 @@ class EmuFormat:
         import emu_harness
         from detectmateservice_b200.component import parse_monitors, select_component_config
         self.mons = parse_monitors(select_component_config(cfg, name))
-        self.lib = C.CDLL(emu_harness.build())
         self.det = emu_harness.EmuDetector([m.key for m in self.mons], table_log2=12)
-        L = self.lib
-        L.emu_set_format.restype = C.c_char_p
-        L.emu_set_format.argtypes = [C.c_void_p, C.c_uint32, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_char_p), C.c_uint32]
-        L.emu_process_format.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
-                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
-        ts = [t if isinstance(t, bytes) else t.encode() for t in templates]
-        fmt = log_format if isinstance(log_format, bytes) else log_format.encode()
-        err = L.emu_set_format(_monitor_array(self.mons), len(self.mons), fmt, b"Content", len(ts), (C.c_char_p * max(1, len(ts)))(*ts),
-                               norm_flags(*norm))
-        if err:
-            raise ValueError(err.decode())
+        self.lib = self.det.lib
+        self.det.set_monitors(_monitor_array(self.mons), len(self.mons))
+        self.det.set_format(log_format, templates, norm_flags(*norm))
 
     def process(self, buf, n_train, with_offsets=False):
         cap = buf.count(b"\n") + 2
@@ -226,10 +217,7 @@ def test_emu_kernel_audit_templates(golden_dir, emu_kernel):
     assert f == wf and s == ws
     assert masks == {i: _mask_of(a, emu.mons) for i, a in enumerate(wa) if a}
     assert sum(wf) >= 5 and bad == 2 and wf[-1] == 1 and ws[-1] == 2.0          # the unterminated last record counts
-    stats = (C.c_uint64 * 40)()
-    emu.lib.emu_get_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
-    emu.lib.emu_get_stats(emu.det.h, stats)
-    assert stats[7] == bad
+    assert emu.stats()["bad_records"] == bad
 
 
 def test_emu_kernel_fuzz_formats(emu_kernel):

@@ -1,11 +1,8 @@
 """LogSchema input (DESIGN.md R-log), CPU tier: the host codec against protobuf's runtime, the device unwrap kernels
 (walk, scan, compact, copy) on the CPU emulator against the protobuf-decode / filter / join oracle, and the
 component's routing with a device stand-in."""
-import ctypes as C
-import os
 import random
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -104,19 +101,7 @@ def test_encode_log_schema_roundtrip_through_protobuf():
 # ------------------------------------------------------------------------------------------ emulator
 def _emu_lib():
     import emu_harness
-    src = os.path.join(emu_harness.EMU, "emu_logs.cpp")
-    so = os.path.join(emu_harness.EMU, "_build", "libemu_logs.so")
-    deps = [src, os.path.join(emu_harness.EMU, "emu_tile.cpp"), os.path.join(emu_harness.EMU, "cuda_emu.h")] + [
-        os.path.join(emu_harness.CSRC, f) for f in os.listdir(emu_harness.CSRC)]
-    if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-DDM_EMU", "-I" + emu_harness.EMU, "-I" + emu_harness.CSRC,
-                               "-shared", "-fPIC", "-pthread", "-o", so, src])
-    lib = C.CDLL(so)
-    lib.emu_logs_unwrap.restype = C.c_int64
-    lib.emu_logs_unwrap.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
-                                    C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    return lib
+    return emu_harness.lib()
 
 
 def _emu_unwrap(lib, msg, delimited, n_train, walk_ctas=2, copy_ctas=2):

@@ -2,7 +2,6 @@
 the kernel source on the CPU emulator (CPU tier) and the real library (GPU tier), both
 against the per-record Python oracle (oracle/nvd.py), which decodes with protobuf's own
 runtime -- an independent codec from the kernel's hand-written field walk."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -69,7 +68,6 @@ def test_emu_record_batch_kernel():
     want_f, want_s, want_m, orc = oracle_run(recs)
     mons = monitors_of(CFG)
     assert [m.alert_key for m in mons] == [m.alert_key for m in orc.monitors]
-    lib = C.CDLL(emu_harness.build())
     det = emu_harness.EmuDetector([m.key for m in mons], table_log2=12)
     arr = (_lib.Monitor * len(mons))()
     for i, m in enumerate(mons):
@@ -82,24 +80,57 @@ def test_emu_record_batch_kernel():
                 arr[i].key[j] = c
         else:
             arr[i].source, arr[i].var_index = 1, m.pos
-    lib.emu_process_records.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint64, C.c_uint32,
-                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    det.set_monitors(arr, len(mons))
     got_f, got_s, got_m = [], [], []
     seen = 0
     for lo in range(0, len(recs), 250):                         # several messages; training spans two of them
         batch = wire.frame_delimited([wire.encode_parser_schema(r) for r in recs[lo:lo + 250]])
         n_train = max(0, min(250, 300 - seen))
         f = np.full(300, 9, np.uint8); s = np.full(300, -1, np.float32); m = np.zeros(300, np.uint32)
-        n_rec, n_an = C.c_uint64(), C.c_uint64()
-        rc = lib.emu_process_records(det.h, arr, len(mons), batch, len(batch), n_train, f.ctypes.data, s.ctypes.data,
-                                     m.ctypes.data, 300, C.byref(n_rec), C.byref(n_an))
+        rc, k, n_an = det.process_records(batch, n_train, f, s, m, 300)
         assert rc == 0
-        k = n_rec.value
         seen += k
         got_f += f[:k].tolist(); got_s += s[:k].tolist(); got_m += m[:k].tolist()
-        assert n_an.value == int(f[:k].sum())
+        assert n_an == int(f[:k].sum())
     assert got_f == want_f and got_s == want_s and got_m == want_m
     assert sum(want_f) > 50
+
+
+def test_emu_frame_split_matches_split_delimited():
+    """The framing split libdmdetect and the emulator share (dm_frame_split) against wire.split_delimited on pbgen
+    batches: length prefixes padded up to 10 bytes are taken, an 11-byte one is refused, as are a prefix the message
+    cuts short and a record that runs past the end; each error at the byte libdmdetect's message names."""
+    import ctypes as C
+    import random
+    import emu_harness
+    from pbgen import Gen, frame, varint
+    lib = emu_harness.lib()
+
+    def split(buf):
+        off, ln, at = np.zeros(len(buf) + 1, np.uint32), np.zeros(len(buf) + 1, np.uint32), C.c_uint64()
+        n = lib.emu_frame_split(buf, len(buf), off.ctypes.data, ln.ctypes.data, len(buf) + 1, C.byref(at))
+        if n < 0:
+            return n, at.value
+        return [buf[o:o + k] for o, k in zip(off[:n].tolist(), ln[:n].tolist())]
+
+    recs, _ = Gen(seed=5).records(300)
+    r = random.Random(5)
+    for overlong_p in (0.0, 0.5, 1.0):
+        buf = frame(recs, r, overlong_p)
+        assert split(buf) == wire.split_delimited(buf) == recs
+    assert split(b"") == wire.split_delimited(b"") == []
+    head = frame(recs[:3])
+    ten = head + varint(3, 10) + b"abc"
+    assert split(ten) == wire.split_delimited(ten) == recs[:3] + [b"abc"]
+    bad = {head + varint(3, 11) + b"abc": (-1, len(head) + 10),        # 11-byte prefix
+           head + b"\x83": (-1, len(head) + 1),                      # prefix cut short by the end of the message
+           head + b"\x83\x80": (-1, len(head) + 2),
+           head + varint(4) + b"abc": (-2, len(head) + 1),            # record runs past the end
+           varint(1 << 40, 10): (-2, 10)}
+    for buf, want in bad.items():
+        with pytest.raises(wire.WireError):
+            wire.split_delimited(buf)
+        assert split(buf) == want, buf
 
 
 @pytest.mark.gpu

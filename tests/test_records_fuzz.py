@@ -2,7 +2,6 @@
 H100 in the GPU tier), the host framing and training split of dm_process_records, and wire.decode_parser_schema,
 all fed with what tests/pbgen.py writes -- non-canonical, mutated and malformed ParserSchema records -- and compared
 record by record with oracle/pbrecords.py (upb decides what is well-formed and what each record holds)."""
-import ctypes as C
 import random
 
 import numpy as np
@@ -75,7 +74,6 @@ class EmuRecords:
         from detectmateservice_b200 import _lib
         self.mons, self.combos = monitors_and_combos(cfg, combo)
         self.det = emu_harness.EmuDetector([b"\x01m%d" % i for i in range(len(self.mons))], table_log2=14)
-        self.lib = self.det.lib
         arr = (_lib.Monitor * len(self.mons))()
         for i, m in enumerate(self.mons):
             arr[i].event_id = m.event_id if m.event_id is not None else 0
@@ -87,37 +85,18 @@ class EmuRecords:
                     arr[i].key[j] = c
             else:
                 arr[i].source, arr[i].var_index = 1, m.pos
-        self.arr = arr
-        self.lib.emu_process_records.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint64, C.c_uint32,
-                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
-                                                 C.POINTER(C.c_uint64)]
-        self.lib.emu_set_combos.argtypes = [C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32]
-
-    def _set_combos(self, on):
-        off, flat = [0], []
-        for mem in (self.combos if on else []):
-            flat += mem
-            off.append(len(flat))
-        member_only = (1 << len(self.mons)) - 1 if on and self.combos else 0
-        self.lib.emu_set_combos(len(off) - 1, (C.c_uint32 * len(off))(*off), (C.c_uint32 * max(1, len(flat)))(*flat),
-                                member_only)
+        self.det.set_monitors(arr, len(self.mons))
+        self.det.set_combos(self.combos, (1 << len(self.mons)) - 1 if self.combos else 0)
 
     def process(self, batch: bytes, n_train: int):
         """-> flags, scores, masks, and the deltas of (bad_records, train_lines, detect_lines, lines)"""
         cap = len(batch) + 1
         f = np.full(cap, 9, np.uint8); s = np.full(cap, -1, np.float32); m = np.full(cap, 0xDEAD, np.uint32)
-        n_rec, n_an = C.c_uint64(), C.c_uint64()
         st0 = self.det.stats()
-        self._set_combos(True)
-        try:
-            rc = self.lib.emu_process_records(self.det.h, self.arr, len(self.mons), batch, len(batch), n_train,
-                                              f.ctypes.data, s.ctypes.data, m.ctypes.data, cap, C.byref(n_rec), C.byref(n_an))
-        finally:
-            self._set_combos(False)
+        rc, k, n_an = self.det.process_records(batch, n_train, f, s, m, cap)
         assert rc == 0
         st1 = self.det.stats()
-        k = n_rec.value
-        assert n_an.value == int(f[:k].sum())
+        assert n_an == int(f[:k].sum())
         d = {w: st1[w] - st0[w] for w in ("bad_records", "train_lines", "detect_lines", "lines")}
         return f[:k], s[:k], m[:k], d
 
