@@ -33,6 +33,11 @@ parser_schema | parser_schema_batch), or named (log_schema | log_schema_batch, n
                 it, so that with a ``log_format`` this component stands where the parser stands.
                 Replies as for ParserSchema input; alerts carry the record's logID.
 
+Alerts of raw-line, LogSchema and ParserSchema batches with at least DEVICE_ALERTS_MIN anomalous records are encoded
+on the device (dm_encode_alerts, rule R-alert in DESIGN.md), byte for byte what the host encoder here writes; the host
+encoder words the rest, every batch the device declines, the two-slot pipelined path and single ParserSchema records
+of B200NewValueDetector.
+
 All detection decisions are taken on the device; there is no CPU path (DeviceDetector
 raises without a GPU).
 """
@@ -356,6 +361,10 @@ class B200NewValueDetector(CoreComponent):
             return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
         if self.det.last_n_anomalies == 0:
             return None
+        if self.det.last_n_anomalies >= self.DEVICE_ALERTS_MIN:
+            enc = self._device_alerts(0, n)
+            if enc is not None:
+                return self._device_reply(enc, bare=False)
         frames = wire.split_delimited(data)
         out = []
         for idx in np.flatnonzero(flags):
@@ -390,6 +399,10 @@ class B200NewValueDetector(CoreComponent):
             return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
         if self.det.last_n_anomalies == 0:
             return None
+        if self.det.last_n_anomalies >= self.DEVICE_ALERTS_MIN:
+            enc = self._device_alerts(0, n)
+            if enc is not None:
+                return self._device_reply(enc, bare=not delimited)
         frames = wire.split_delimited(data) if delimited else [data]
         raw_keys = [m.key for m in self.monitors]
         out = []
@@ -438,12 +451,16 @@ class B200NewValueDetector(CoreComponent):
     # scripts/e2e_pieces.py measures one call against 2 / 4 / 8 / 12 MiB pieces on the machine at hand.
     PIPE_MIN_BYTES = 24 << 20
     PIPE_PIECE_BYTES = 12 << 20
-    # Batches with at least this many anomalous records have their alerts encoded on the device (dm_encode_alerts).  On
+    # Batches with at least this many anomalous records have their alerts encoded on the device (dm_encode_alerts), raw
+    # lines, LogSchema and ParserSchema alike.  On
     # one H100 (700 W), 64k-record messages, process() median [range] in ms, host encoder against device encoder: 1 alert
     # 0.60 against 0.59 [0.57-0.62], 4 alerts 0.65 [0.56-0.75] against 0.58 [0.55-0.61], 8 alerts 0.61 [0.59-0.76]
     # against 0.54 [0.53-0.60], 16 alerts 0.92 against 0.58 (scripts/alerts_bench.py, DESIGN.md section 5.3).  Below 8
     # the two overlap, and a record with a long value once made one alert slower on the device (0.77 against 0.60), so
-    # the device takes over where it was ahead beyond the spread.
+    # the device takes over where it was ahead beyond the spread.  64k-record LogSchema / ParserSchema batches on the
+    # same card were ahead on the device from 1 alert on (LogSchema 85 against 6.4 ms, ParserSchema 63 against 8.8 ms,
+    # scripts/record_alerts_bench.py): there the host path splits the whole message first.  Small batches were not
+    # measured, so the three inputs share this threshold.
     DEVICE_ALERTS_MIN = 8
 
     def _detect_pipelined(self, data):
@@ -506,14 +523,7 @@ class B200NewValueDetector(CoreComponent):
         if anomalies is None and n_anom >= self.DEVICE_ALERTS_MIN:
             enc = self._device_alerts(base, n)
             if enc is not None:
-                blob, count = enc
-                self.n_alerts += count
-                if not count:
-                    return None
-                if n == 1 and not force_delimited:
-                    _ln, pos = wire._read_varint(blob, 0)              # one record in, one bare DetectorSchema out
-                    return blob[pos:]
-                return blob
+                return self._device_reply(enc, bare=n == 1 and not force_delimited)
         if anomalies is None:
             anomalies = self.det.anomalies()
         out = []
@@ -571,9 +581,10 @@ class B200NewValueDetector(CoreComponent):
         return sorted(by_key.items())
 
     def _device_alerts(self, first_log_id: int, n_records: int) -> Optional[Tuple[bytes, int]]:
-        """The alerts of the last raw-line batch encoded on the device (DESIGN.md R-alert): (varint-delimited
-        DetectorSchemas, count), or None when the host encodes them -- the device declined the batch, the handle has no
-        encoder (a stand-in), or an ID does not fit the device's 64-bit integers."""
+        """The alerts of the last batch -- raw lines, LogSchema or ParserSchema records -- encoded on the device (DESIGN.md
+        R-alert): (varint-delimited DetectorSchemas, count), or None when the host encodes them -- the device declined
+        the batch, the handle has no encoder (a stand-in), or an ID does not fit the device's 64-bit integers.
+        first_log_id numbers raw lines; the other two carry their records' logIDs and pass 0."""
         det = self.det
         if not hasattr(det, "encode_alerts"):
             return None
@@ -590,6 +601,18 @@ class B200NewValueDetector(CoreComponent):
                                  time_capture=names.index("Time") if "Time" in names else None)
             self._alert_sig = sig
         return det.encode_alerts(first_log_id, first_alert_id, now)
+
+    def _device_reply(self, enc: Tuple[bytes, int], bare: bool) -> Optional[bytes]:
+        """The reply made of _device_alerts' result: None without alerts, the one DetectorSchema without its length
+        prefix when one record came in bare, else the varint-delimited DetectorSchemas."""
+        blob, count = enc
+        self.n_alerts += count
+        if not count:
+            return None
+        if bare:
+            _ln, pos = wire._read_varint(blob, 0)
+            return blob[pos:]
+        return blob
 
     def _description(self) -> str:
         return f"{self.detector_id} detects values not encountered in training as anomalies."

@@ -1,8 +1,9 @@
-// dm_kernels_alerts.cuh -- the DetectorSchema alerts of a raw-line batch, encoded on the device (rule R-alert, DESIGN.md).
+// dm_kernels_alerts.cuh -- the DetectorSchema alerts of the last batch, encoded on the device (rule R-alert, DESIGN.md).
 //
-// The host path (component.py: _line_alerts / _detector_schema / wire.encode_detector_schema) is the specification: for
-// the last dm_process_lines batch in key=value mode these kernels write, byte for byte, the varint-delimited
-// DetectorSchemas the host writes for it.  Launches, with no host round trip in between:
+// The host path (component.py: _process_lines_one / _process_logs / _process_record_batch, _detector_schema,
+// wire.encode_detector_schema) is the specification: for the last dm_process_lines, dm_process_logs or
+// dm_process_records batch these kernels write, byte for byte, the varint-delimited DetectorSchemas the host writes for
+// it.  Launches for raw lines, with no host round trip in between:
 //   dm_k_alert_mark     one thread per anomaly entry: mark its record
 //   dm_alert_scan       exclusive scan of the marks: the rank of each anomalous record, in record order; the count
 //   dm_k_alert_gather   one thread per anomaly entry: OR its mask into its record's merged mask (the stream kernel appends
@@ -13,6 +14,11 @@
 //   dm_k_alert_write    one thread per anomalous record: the same walk as dm_k_alert_size, writing
 // In log_format mode dm_k_alert_format<NORM, false / true> takes the place of the size / write kernels: it re-runs the
 // header and template chains with the matcher's own device functions (dm_fmtl_*, dm_kernels_format.cuh) before the walk.
+// LogSchema batches (DMA_LOGS) take the same launches: dm_k_logs_scatter has already rewritten the anomaly list to
+// record indices, and a record's text is its line of the compacted buffer, so only dm_k_alert_gather (where the text
+// starts) and the logID (the last field 2 of the payload, dma_log_id) differ.  ParserSchema batches (DMA_RECORDS) have
+// no anomaly list: dm_k_alert_mark_records / dm_k_alert_gather_records take the per-record flags and masks, and
+// dm_k_alert_records<false / true> walks each anomalous record once with the detection kernels' own walk.
 // A record is walked by one thread; a record of max_batch_bytes is walked by one thread too, slowly but correctly.
 #pragma once
 #include "dm_device.cuh"
@@ -25,6 +31,9 @@
 #define DMA_POOL 16384                             // bytes of constant text (fields 1-3, field 10, alert keys)
 #define DMA_MSG DM_MAX_KEYS                        // key slot of "msg", the Time source of R-tok L7
 #define DMA_NONE 0xFFu
+#define DMA_LINES 0u                               // DmAlertArgs::src: the batch came from dm_process_lines,
+#define DMA_LOGS 1u                                //   dm_process_logs
+#define DMA_RECORDS 2u                             //   or dm_process_records
 
 // What dm_set_alert_format fixes: everything of a DetectorSchema that does not depend on the record or the call.
 struct DmAlertFmt {
@@ -72,6 +81,16 @@ struct DmAlertArgs {
     unsigned long long out_cap;
     const DmFormat* efmt;                          // log_format mode: the matcher's format, keeping the Time capture too
     uint8_t* nbuf;                                 //   R-norm: the message-sized scratch the Content is normalised into
+    uint32_t src = DMA_LINES;                      // the batch's input; for DMA_LOGS buf is the compacted texts, scores
+                                                   // and anomaly lines are per record
+    const uint8_t* pay = nullptr;                  // DMA_LOGS / DMA_RECORDS: the caller's message; per record the offset
+    const uint32_t* pay_off = nullptr;             //   and length of its payload
+    const uint32_t* pay_len = nullptr;
+    const uint32_t* log_line = nullptr;            // DMA_LOGS: per record its line of buf, per line where it starts
+    const uint32_t* log_dst = nullptr;
+    const uint8_t* flags = nullptr;                // DMA_RECORDS: per record its flag and mask, and the monitors
+    const uint32_t* masks = nullptr;
+    const DmMonitors* mons = nullptr;
 };
 
 // ---------------------------------------------------------------------------------------------- exclusive scan
@@ -161,7 +180,24 @@ __global__ void __launch_bounds__(DMA_THREADS) dm_k_alert_gather(DmAlertArgs a) 
         const uint32_t r = a.rank[e.line];
         atomicOr(&a.rec_mask[r], e.mask);
         a.rec_line[r] = e.line;                    // (every entry of a record carries the same line and offset)
-        a.rec_off[r] = e.offset;
+        a.rec_off[r] = a.src == DMA_LOGS ? a.log_dst[a.log_line[e.line]] : e.offset;
+    }
+}
+
+// ParserSchema batches: the flags of dm_process_records mark the anomalous records, their masks are already merged.
+__global__ void __launch_bounds__(DMA_THREADS) dm_k_alert_mark_records(DmAlertArgs a) {
+    for (uint64_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.n_lines; r += gridDim.x * blockDim.x)
+        a.rank[r] = a.flags[r] ? 1u : 0u;
+}
+
+__global__ void __launch_bounds__(DMA_THREADS) dm_k_alert_gather_records(DmAlertArgs a) {
+    for (uint64_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.n_lines; r += gridDim.x * blockDim.x) {
+        if (!a.flags[r]) continue;
+        const uint32_t k = a.rank[r];
+        if (k >= a.n_entries) { atomicOr(&a.ahdr->declined, 1u); continue; }     // (the host sized n_entries from the count)
+        a.rec_line[k] = (uint32_t)r;
+        a.rec_mask[k] = a.masks[r];
+        a.rec_off[k] = a.pay_off[r];
     }
 }
 
@@ -274,15 +310,20 @@ __device__ __forceinline__ unsigned long long dma_fields(const DmAlertFmt& F, co
 // rounded float of s never reaches it); `now` for an empty s and for an s holding a byte no float literal can hold
 // (CPython's float() of bytes accepts only ASCII white space, digits, '.', '+', '-', 'e', '_' and the letters of inf,
 // infinity and nan, in either case).  False for every other string: the record declines.
-__device__ __forceinline__ bool dma_time(const uint8_t* s, uint32_t n, long long now, long long* ts) {
-    bool foreign = n == 0;
+// str: s is the UTF-8 of a str (a ParserSchema map value), and float() of a str also takes Unicode decimal digits and
+// white space.  An ASCII byte outside the alphabet above still proves `now` (every other character maps to one that
+// fails the parse), but a string without one that holds a byte >= 0x80 declines.
+__device__ __forceinline__ bool dma_time(const uint8_t* s, uint32_t n, long long now, long long* ts, bool str = false) {
+    bool foreign = n == 0, wide = false;
     for (uint32_t j = 0; j < n && !foreign; ++j) {
+        if (str && s[j] >= 0x80u) { wide = true; continue; }
         const uint8_t c = s[j] | ((s[j] >= 'A' && s[j] <= 'Z') ? 0x20u : 0u);
         foreign = !((c >= '0' && c <= '9') || c == '.' || c == '+' || c == '-' || c == '_' || c == ' ' ||
                     (c >= 0x09u && c <= 0x0Du) || c == 'e' || c == 'i' || c == 'n' || c == 'f' || c == 't' ||
                     c == 'y' || c == 'a');
     }
     if (foreign) { *ts = now; return true; }
+    if (wide) return false;
     uint32_t i = 0;
     long long v = 0;
     while (i < n && s[i] >= '0' && s[i] <= '9') { v = v * 10 + (s[i] - '0'); ++i; if (i > 10) return false; }
@@ -305,6 +346,8 @@ struct DmaRec {
     DmaSpan span[DM_MAX_KEYS + 1];
     uint8_t pick[DM_MAX_KEYS];                     // per alert key: the mask bit that supplies it, DMA_NONE if absent
     long long ts;                                  // extractedTimestamps[0]
+    const uint8_t* lid;                            // logIDs[0]: [lid, + lid_n) (LogSchema, ParserSchema), or nullptr:
+    uint32_t lid_n;                                //   the decimal first_log_id + line (raw lines)
 };
 
 __device__ __forceinline__ void dma_value(DmaOut& w, const DmaRec& R, uint32_t k) {
@@ -339,7 +382,6 @@ __device__ __forceinline__ void dma_body(DmaOut& x, const DmAlertArgs& a, const 
     const DmAlertFmt& F = *a.fmt;
     const long long aid = a.first_alert_id + (long long)r;
     const unsigned long long aid_mag = aid < 0 ? 0ull - (unsigned long long)aid : (unsigned long long)aid;
-    const unsigned long long lid = a.first_log_id + R.line;
     x.bytes(F.pool, F.head_len);                                     // 1 __version__, 2 detectorID, 3 detectorType
     x.byte(0x22);                                                    // 4 alertID
     x.varint(dma_dec_len(aid_mag) + (aid < 0 ? 1u : 0u));
@@ -348,8 +390,14 @@ __device__ __forceinline__ void dma_body(DmaOut& x, const DmAlertArgs& a, const 
     x.byte(0x28);                                                    // 5 detectionTimestamp
     x.varint((unsigned long long)a.now);
     x.byte(0x32);                                                    // 6 logIDs
-    x.varint(dma_dec_len(lid));
-    x.dec(lid);
+    if (R.lid) {
+        x.varint(R.lid_n);
+        x.bytes(R.lid, R.lid_n);
+    } else {
+        const unsigned long long lid = a.first_log_id + R.line;
+        x.varint(dma_dec_len(lid));
+        x.dec(lid);
+    }
     uint32_t sb;                                                     // 8 score
     memcpy(&sb, &a.scores[R.line], 4);
     x.byte(0x45);
@@ -402,12 +450,38 @@ __device__ __forceinline__ void dma_finish(const DmAlertArgs& a, uint32_t r, con
     else w.n += c.n;
 }
 
+// logIDs[0] of the record R.line: nothing to find for a raw line (R.lid = nullptr, the decimal number); for a LogSchema
+// record the last `logID` (field 2, LEN) of its payload, "" when it has none, as protobuf reads it.  False where the
+// payload does not walk (a record the unwrap kernels accepted always does).
+__device__ __forceinline__ bool dma_log_id(const DmAlertArgs& a, DmaRec& R) {
+    R.lid = nullptr;
+    R.lid_n = 0;
+    if (a.src != DMA_LOGS) return true;
+    uint32_t pos = a.pay_off[R.line];
+    const uint32_t end = pos + a.pay_len[R.line];
+    R.lid = a.pay + pos;
+    while (pos < end) {
+        uint32_t field, wt;
+        if (!dm_pb_tag(a.pay, pos, end, field, wt)) return false;
+        if (wt != 2) {
+            if (!dm_pb_skip(a.pay, pos, end, wt)) return false;
+            continue;
+        }
+        uint64_t len;
+        if (!dm_pb_varint(a.pay, pos, end, len) || len > (uint64_t)(end - pos)) return false;
+        if (field == 2) { R.lid = a.pay + pos; R.lid_n = (uint32_t)len; }
+        pos += (uint32_t)len;
+    }
+    return true;
+}
+
 // Anomalous record r of a key=value batch: its varint-delimited DetectorSchema, written to w (or counted).  False: the
 // record declines.
 __device__ bool dma_emit(const DmAlertArgs& a, uint32_t r, DmaOut& w) {
     const DmAlertFmt& F = *a.fmt;
     DmaRec R;
     R.line = a.rec_line[r];
+    if (!dma_log_id(a, R)) return false;
     const unsigned long long off = a.rec_off[r];
     R.s = a.buf + off;
     R.ns = nullptr;
@@ -520,11 +594,72 @@ __global__ void __launch_bounds__(DM_FMTL_THREADS) dm_k_alert_format(DmAlertArgs
             }
         }
         R.ts = a.now;
-        bool ok = true;
-        if (F.time_cap != DMA_NONE && hok && F.time_cap < n_hcaps) {
+        bool ok = dma_log_id(a, R);
+        if (ok && F.time_cap != DMA_NONE && hok && F.time_cap < n_hcaps) {
             const uint2 tc = hcap[(uint32_t)__popc(f.chain_need[0] & ((1u << F.time_cap) - 1u)) * DM_FMTL_THREADS];
             ok = dma_time(a.buf + tc.x, tc.y, a.now, &R.ts);
         }
+        if (WRITE) {
+            DmaOut w{a.out, a.size[r]};
+            dma_finish(a, r, R, w);
+        } else {
+            unsigned long long bytes = 0;
+            if (ok) {
+                DmaOut w{nullptr, 0};
+                dma_finish(a, r, R, w);
+                bytes = w.n;
+            } else {
+                atomicOr(&a.ahdr->declined, 1u);
+            }
+            a.size[r] = bytes;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- ParserSchema batches
+// One thread per anomalous record: the detection kernels' walk (dm_pb_walk_record_t) once more, now also keeping the
+// logID and the Time entry.  Monitor k's value is what that walk found for it (a monitor is only flagged where the
+// record has its value and, for an event monitor, its EventID); Time is logFormatVariables["Time"] as a str, absent =
+// the clock.  !WRITE: the size pass (and declines); WRITE: the write pass.
+template <bool WRITE>
+__global__ void __launch_bounds__(DMA_THREADS) dm_k_alert_records(DmAlertArgs a) {
+    __shared__ DmMonitors sm;
+    {
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(a.mons);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(&sm);
+        for (uint32_t i = threadIdx.x; i < sizeof(DmMonitors) / 4; i += blockDim.x) dst[i] = src[i];
+    }
+    __syncthreads();
+    const DmAlertFmt& F = *a.fmt;
+    const uint32_t n = a.ahdr->n_alerts;
+    if (WRITE && (a.ahdr->declined || a.ahdr->total > a.out_cap)) return;
+    const uint32_t lim = WRITE ? n : a.n_entries;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < lim; r += gridDim.x * blockDim.x) {
+        if (r >= n) { a.size[r] = 0; continue; }
+        DmaRec R;
+        R.line = a.rec_line[r];
+        R.s = a.pay;
+        R.ns = nullptr;
+        const uint32_t pos = (uint32_t)a.rec_off[r];
+        uint32_t vp[DM_MAX_KEYS], vl[DM_MAX_KEYS], present = 0;
+        int32_t eid = 0;
+        bool has_eid = false;
+        DmPbMeta m;
+        m.lid_p = pos; m.lid_l = 0; m.time_p = pos; m.time_l = 0; m.has_time = false;
+        bool ok = dm_pb_walk_record_t<true>(a.pay, pos, pos + a.pay_len[R.line], sm, vp, vl, present, eid, has_eid, &m);
+        dma_pick(F, a.rec_mask[r], R);
+        R.found = 0;
+        for (uint32_t k = 0; k < F.n_keys; ++k) {
+            if (!(present >> k & 1u)) continue;
+            R.span[k].b = vp[k];
+            R.span[k].e = vp[k] + vl[k];
+            R.span[k].nrm = 0;
+            R.found |= 1ull << k;
+        }
+        R.lid = a.pay + m.lid_p;
+        R.lid_n = m.lid_l;
+        R.ts = a.now;
+        if (ok && m.has_time) ok = dma_time(a.pay + m.time_p, m.time_l, a.now, &R.ts, true);
         if (WRITE) {
             DmaOut w{a.out, a.size[r]};
             dma_finish(a, r, R, w);

@@ -73,9 +73,18 @@ DM_HD bool dm_pb_string_field(uint32_t f) { return f <= 9u && ((0x3EEu >> f) & 1
 // them: the last EventID wins, variables[i] is the i-th field 6, logFormatVariables[key] the last entry with that key.
 // A map entry holding anything but LEN fields 1 and 2 is dropped, as protobuf's runtime drops it (its key and value are
 // still checked for UTF-8); an absent key or value reads as "".
-__device__ __forceinline__ bool dm_pb_walk_record(const uint8_t* __restrict__ buf, uint32_t pos, const uint32_t end,
-                                                  const DmMonitors& sm, uint32_t* vp, uint32_t* vl, uint32_t& present,
-                                                  int32_t& eid, bool& has_eid) {
+// META (the alert encoder, dm_kernels_alerts.cuh): *meta also gets the last logID (field 8 as LEN) and the last
+// logFormatVariables["Time"], by the same rules; the detection kernels walk with META = false.
+struct DmPbMeta {
+    uint32_t lid_p, lid_l;                 // logID, [lid_p, + lid_l); lid_l = 0 when absent
+    uint32_t time_p, time_l;
+    bool has_time;
+};
+
+template <bool META>
+__device__ __forceinline__ bool dm_pb_walk_record_t(const uint8_t* __restrict__ buf, uint32_t pos, const uint32_t end,
+                                                    const DmMonitors& sm, uint32_t* vp, uint32_t* vl, uint32_t& present,
+                                                    int32_t& eid, bool& has_eid, DmPbMeta* meta) {
     uint32_t var_idx = 0;
     while (pos < end) {
         uint32_t field, wt;
@@ -95,6 +104,7 @@ __device__ __forceinline__ bool dm_pb_walk_record(const uint8_t* __restrict__ bu
         if (!dm_pb_varint(buf, pos, end, len64) || len64 > (uint64_t)(end - pos)) return false;
         const uint32_t len = (uint32_t)len64;
         if (dm_pb_string_field(field) && !dm_utf8_ok(buf + pos, len)) return false;
+        if (META && field == 8) { meta->lid_p = pos; meta->lid_l = len; }
         if (field == 6) {
             for (uint32_t k = 0; k < sm.n; ++k)
                 if (sm.m[k].source == 1 && sm.m[k].var_index == var_idx) { vp[k] = pos; vl[k] = len; present |= 1u << k; }
@@ -119,6 +129,9 @@ __device__ __forceinline__ bool dm_pb_walk_record(const uint8_t* __restrict__ bu
                 p += (uint32_t)l2;
             }
             if (!foreign) {
+                if (META && kl == 4 && buf[kp] == 'T' && buf[kp + 1] == 'i' && buf[kp + 2] == 'm' && buf[kp + 3] == 'e') {
+                    meta->time_p = xp; meta->time_l = xl; meta->has_time = true;
+                }
                 for (uint32_t k = 0; k < sm.n; ++k) {
                     if (sm.m[k].source != 0 || sm.m[k].key_len != kl) continue;
                     bool eq = true;
@@ -131,6 +144,12 @@ __device__ __forceinline__ bool dm_pb_walk_record(const uint8_t* __restrict__ bu
         pos += len;
     }
     return true;
+}
+
+__device__ __forceinline__ bool dm_pb_walk_record(const uint8_t* __restrict__ buf, uint32_t pos, const uint32_t end,
+                                                  const DmMonitors& sm, uint32_t* vp, uint32_t* vl, uint32_t& present,
+                                                  int32_t& eid, bool& has_eid) {
+    return dm_pb_walk_record_t<false>(buf, pos, end, sm, vp, vl, present, eid, has_eid, nullptr);
 }
 
 // phase 2: mark each record well-formed (flags[r] = 1) or not, for dm_k_records_bound;

@@ -57,6 +57,9 @@ extern "C" uint64_t dm_table_key(uint32_t field, const uint8_t* value, uint32_t 
 // ---------------------------------------------------------------------------------------
 // handle
 // ---------------------------------------------------------------------------------------
+// Where the last batch came from (dm_handle::last_src): the batches dm_encode_alerts can word, or none of them.
+enum { DM_SRC_NONE = 0, DM_SRC_LINES, DM_SRC_LOGS, DM_SRC_RECORDS };
+
 struct dm_handle {
     int device = 0;
     int sm_count = 0;
@@ -115,7 +118,8 @@ struct dm_handle {
     // DetectorSchema alerts on the device (dm_set_alert_format / dm_encode_alerts), allocated by dm_set_alert_format
     const uint8_t* last_buf = nullptr;   // the last dm_process_lines batch as its kernels read it, and its scores
     const float* last_scores = nullptr;
-    bool last_was_lines = false;         // the last batch came from dm_process_lines itself
+    uint32_t last_src = DM_SRC_NONE;     // where the last batch came from: what dm_encode_alerts can word
+    uint32_t last_n_records = 0;         // its records (dm_process_records)
     DmAlertFmt* d_afmt = nullptr;
     DmAlertHeader* d_ahdr = nullptr;
     DmAlertHeader* h_ahdr = nullptr;     // pinned
@@ -468,7 +472,7 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     if (!stream_kernel) h->dmx.chain_stream = nullptr;     // (a launch that is not the stream kernel's ends the overlap chain)
     h->last_buf = d_buf;
     h->last_scores = d_scores;
-    h->last_was_lines = true;
+    h->last_src = DM_SRC_LINES;
 
     const bool want_sync = host_out || n_lines_out || n_anomalies_out;
     if (!want_sync) return DM_OK;
@@ -523,7 +527,7 @@ extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blo
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
-    h->last_was_lines = false;
+    h->last_src = DM_SRC_NONE;
     if (n_values > h->vals_cap) {
         if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
         h->vals_cap = std::max<uint64_t>(2ull * n_values, 4096);
@@ -720,7 +724,7 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
-    h->last_was_lines = false;
+    h->last_src = DM_SRC_NONE;
     if (2ull * n_records + 2 > 3ull * h->vals_cap + 1) {
         if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
         h->vals_cap = std::max<uint64_t>(2ull * n_records, 4096);
@@ -773,6 +777,8 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     if (rc != DM_OK) return rc;
     if (n_records_out) *n_records_out = n_records;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    h->last_src = DM_SRC_RECORDS;
+    h->last_n_records = n_records;
     return DM_OK;
 }
 
@@ -883,13 +889,13 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
         uint64_t n_lines = 0, n_anoms = 0;
         rc = dm_process_lines(h, h->d_logs_text, lh.total_bytes, 1, lh.n_train, nullptr, nullptr, 0, 0, &n_lines, &n_anoms, st);
         dm_break_chain(h, st);
-        h->last_was_lines = false;                            // (its anomaly list is rewritten to records below)
+        h->last_src = DM_SRC_NONE;                            // (its anomaly list is rewritten to records below)
         if (rc != DM_OK) return rc;
         if (n_lines != lh.n_lines)
             return dm_fail(DM_ERR_STATE, "the line path found %llu records in %llu unwrapped texts", (unsigned long long)n_lines, (unsigned long long)lh.n_lines);
     } else {
         DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
-        h->last_was_lines = false;
+        h->last_src = DM_SRC_NONE;
     }
     const int grid_s = (int)std::max<uint32_t>(1, std::min<uint32_t>(std::max<uint32_t>(tiles, h->anomaly_cap / DML_THREADS), (uint32_t)h->sm_count * 8));
     dm_k_logs_scatter<<<grid_s, DML_THREADS, 0, st>>>(a, h->d_flags, h->d_scores, d_rflags, d_rscores, h->d_anoms, h->anomaly_cap,
@@ -903,6 +909,8 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     if (n_records_out) *n_records_out = n_records;
     if (n_malformed_out) *n_malformed_out = n_records - lh.n_lines;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    h->last_src = DM_SRC_LOGS;                                // (the line path left last_buf / last_nbytes: the texts)
+    h->last_scores = d_rscores;
     return DM_OK;
 }
 
@@ -988,15 +996,25 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     if (!h || !out_len || !n_alerts || !declined) return dm_fail(DM_ERR_ARG, "NULL argument");
     if (out_cap && !out) return dm_fail(DM_ERR_ARG, "out is NULL");
     if (!h->d_afmt || !h->d_aout) return dm_fail(DM_ERR_STATE, "dm_set_alert_format has not been called");
-    if (!h->last_was_lines) return dm_fail(DM_ERR_STATE, "the last batch did not come from dm_process_lines");
+    if (h->last_src == DM_SRC_NONE)
+        return dm_fail(DM_ERR_STATE, "the last batch did not come from dm_process_lines, dm_process_logs or dm_process_records");
     *out_len = 0;
     *n_alerts = 0;
     *declined = 0;
     int rc = dm_sync(h, nullptr, nullptr);
     if (rc != DM_OK) return rc;
-    const uint32_t entries = std::min(h->h_hdr->anomaly_list_count, h->anomaly_cap);
-    const uint64_t n_lines = h->h_hdr->n_lines;
-    if (entries == 0 || n_lines == 0) return DM_OK;
+    const uint32_t src = h->last_src;
+    const bool records = src == DM_SRC_RECORDS;
+    // raw lines and LogSchema: the anomaly list (in record space after dm_k_logs_scatter); ParserSchema: the flags
+    const uint64_t n_lines = records ? h->last_n_records : h->h_hdr->n_lines;
+    const uint64_t n_flagged = records ? h->h_hdr->n_anomalies : std::min(h->h_hdr->anomaly_list_count, h->anomaly_cap);
+    if (n_flagged == 0 || n_lines == 0) return DM_OK;
+    if (n_flagged > h->anomaly_cap) {                         // more anomalous records than the per-record arrays hold
+        *n_alerts = n_flagged;
+        *declined = 1;
+        return DM_OK;
+    }
+    const uint32_t entries = (uint32_t)n_flagged;
     cudaStream_t st = h->last_stream;
     dm_break_chain(h, st);
     const uint64_t lines = h->max_lines + 1, recs = (uint64_t)h->anomaly_cap + 1;
@@ -1012,23 +1030,38 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     a.ahdr = h->d_ahdr; a.first_log_id = first_log_id; a.first_alert_id = first_alert_id; a.now = now;
     a.out = h->d_aout; a.out_cap = std::min(out_cap, h->alert_cap);
     a.efmt = h->d_efmt; a.nbuf = h->d_norm;
+    if (src == DM_SRC_LOGS) {
+        float* rscores;
+        uint8_t* rflags;
+        const DmLogsArgs la = dm_logs_args(h, &rscores, &rflags);
+        a.src = DMA_LOGS; a.pay = h->d_in; a.pay_off = la.rec_off; a.pay_len = la.rec_len;
+        a.log_line = la.rec_line; a.log_dst = la.line_dst;
+    } else if (records) {
+        a.src = DMA_RECORDS; a.pay = h->d_in; a.pay_off = h->d_vals; a.pay_len = h->d_vals + n_lines;
+        a.scores = h->d_scores; a.flags = h->d_flags; a.masks = h->d_masks; a.mons = h->d_mons;
+    }
     // log_format mode: the size and write passes re-run the matcher (one thread per record, DM_FMTL_THREADS per CTA)
-    const bool fmt = h->fmt_set, norm = h->fmt_norm;
+    const bool fmt = h->fmt_set && !records, norm = h->fmt_norm;
     if (fmt && !h->d_efmt) return dm_fail(DM_ERR_STATE, "no log_format for the alert encoder");
     const size_t fsmem = (size_t)2 * h->efmt_slots * DM_FMTL_THREADS * sizeof(uint2);
     const int fgrid = (int)std::max<uint32_t>(1, std::min<uint32_t>((entries + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS, (uint32_t)h->sm_count * 32));
     const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>((entries + DMA_THREADS - 1) / DMA_THREADS, (uint32_t)h->sm_count * 8));
+    const int rgrid = (int)std::max<uint64_t>(1, std::min<uint64_t>((n_lines + DMA_THREADS - 1) / DMA_THREADS, (uint64_t)h->sm_count * 8));
     DM_CUDA(cudaMemsetAsync(h->d_ahdr, 0, sizeof(DmAlertHeader), st));
     DM_CUDA(cudaMemsetAsync(a.rank, 0, n_lines * 4, st));
     DM_CUDA(cudaMemsetAsync(a.rec_mask, 0, (uint64_t)entries * 4, st));
-    dm_k_alert_mark<<<grid, DMA_THREADS, 0, st>>>(a);
+    if (records) dm_k_alert_mark_records<<<rgrid, DMA_THREADS, 0, st>>>(a);
+    else dm_k_alert_mark<<<grid, DMA_THREADS, 0, st>>>(a);
     dm_alert_scan<uint32_t>(a.rank, n_lines, (uint32_t*)tile_sums, &h->d_ahdr->n_alerts, st);
-    dm_k_alert_gather<<<grid, DMA_THREADS, 0, st>>>(a);
-    if (!fmt) dm_k_alert_size<<<grid, DMA_THREADS, 0, st>>>(a);
+    if (records) dm_k_alert_gather_records<<<rgrid, DMA_THREADS, 0, st>>>(a);
+    else dm_k_alert_gather<<<grid, DMA_THREADS, 0, st>>>(a);
+    if (records) dm_k_alert_records<false><<<grid, DMA_THREADS, 0, st>>>(a);
+    else if (!fmt) dm_k_alert_size<<<grid, DMA_THREADS, 0, st>>>(a);
     else if (norm) dm_k_alert_format<true, false><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
     else dm_k_alert_format<false, false><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
     dm_alert_scan<unsigned long long>(a.size, entries, tile_sums, &h->d_ahdr->total, st);
-    if (!fmt) dm_k_alert_write<<<grid, DMA_THREADS, 0, st>>>(a);
+    if (records) dm_k_alert_records<true><<<grid, DMA_THREADS, 0, st>>>(a);
+    else if (!fmt) dm_k_alert_write<<<grid, DMA_THREADS, 0, st>>>(a);
     else if (norm) dm_k_alert_format<true, true><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
     else dm_k_alert_format<false, true><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
     h->launches += 10;
@@ -1089,7 +1122,7 @@ extern "C" int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t n
     DM_CUDA(cudaEventRecord(sl.ev_in, h->st_in));
     cudaStream_t st = h->stream;                       // ONE compute stream: submission order = processing order
     h->last_stream = st;
-    h->last_was_lines = false;
+    h->last_src = DM_SRC_NONE;
     DM_CUDA(cudaStreamWaitEvent(st, sl.ev_in, 0));
     if (nbytes == 0) DM_CUDA(cudaMemsetAsync(sl.d_hdr, 0, sizeof(DmBatchHeader), st));
     const int launched = dmx_launch(&h->dmx, sl.d_in, nbytes, n_train_lines, h->table, sl.d_flags, sl.d_scores, h->max_lines, sl.d_anoms,
@@ -1239,7 +1272,7 @@ extern "C" int dm_import_known(dm_handle* h, const uint64_t* keys, uint64_t n) {
     DM_CUDA(cudaMemcpy(d_tmp, keys, n * sizeof(unsigned long long), cudaMemcpyHostToDevice));
     DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), h->last_stream));
     dm_break_chain(h, h->last_stream);
-    h->last_was_lines = false;
+    h->last_src = DM_SRC_NONE;
     dm_k_insert_keys<<<std::max(1, (int)std::min<uint64_t>((n + 255) / 256, 1024)), 256, 0, h->last_stream>>>(h->table, d_tmp, n, &h->d_hdr->error);
     DM_CUDA(cudaGetLastError());
     int rc = dm_sync(h, nullptr, nullptr);

@@ -298,8 +298,9 @@ class DeviceDetector:
             self._pin_alerts = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
 
     def encode_alerts(self, first_log_id: int, first_alert_id: int, now: int) -> Optional[Tuple[bytes, int]]:
-        """The varint-delimited DetectorSchemas of the last process_lines() batch (dm_encode_alerts) and their count, or
-        None when the device declines the batch (the caller then encodes it on the host)."""
+        """The varint-delimited DetectorSchemas of the last process_lines(), process_logs() or process_records() batch
+        (dm_encode_alerts) and their count, or None when the device declines the batch (the caller then encodes it on
+        the host).  first_log_id numbers raw lines only; LogSchema and ParserSchema alerts carry the record's logID."""
         out_len, n, declined = C.c_uint64(), C.c_uint64(), C.c_int()
         buf = self._pin_alerts
         _lib.check(self._lib.dm_encode_alerts(self._h, int(first_log_id), int(first_alert_id), int(now), buf.data_ptr(),

@@ -244,9 +244,10 @@ int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delim
                     uint8_t* flags_out, float* scores_out, uint64_t out_cap,
                     uint64_t* n_records_out, uint64_t* n_malformed_out, uint64_t* n_anomalies_out);
 
-/* DetectorSchema alerts of a raw-line batch, encoded on the device (rule R-alert, DESIGN.md): the bytes the component's
- * host encoder writes for the same batch (component.py _line_alerts / _format_alerts / _detector_schema,
- * wire.encode_detector_schema), in key=value mode and in log_format mode (dm_set_format[_ex]).
+/* DetectorSchema alerts of the last batch, encoded on the device (rule R-alert, DESIGN.md): the bytes the component's
+ * host encoder writes for the same batch (component.py _process_lines_one / _process_logs / _process_record_batch,
+ * _detector_schema, wire.encode_detector_schema), for raw lines and LogSchema records in key=value mode and in
+ * log_format mode (dm_set_format[_ex]), and for ParserSchema records.
  * dm_set_alert_format fixes what does not change from call to call and allocates, once, the device buffers, of which
  * the output buffer holds out_cap bytes:
  *   strings / string_lens : n_strings strings, concatenated: __version__, detectorID, detectorType, description, then
@@ -257,21 +258,28 @@ int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delim
  *                           combo_members[combo_off[c], combo_off[c + 1]) ("Unknown value combination: ('<v1>', ...)").
  *                           Monitor k's value: key=value mode, the first true field of key k of dm_create (R-tok
  *                           L2-L6); log_format mode, its header capture verbatim or its template variable (under
- *                           R-norm a slice of the normalised Content);
+ *                           R-norm a slice of the normalised Content); ParserSchema records, the value the
+ *                           monitor of dm_set_monitors reads (logFormatVariables[key], last entry wins, or
+ *                           variables[i]);
  *   time_capture          : log_format mode: the header capture whose text is the record's Time, 0xFFFFFFFF = none
  *                           (key=value mode always takes msg=audit(<Time>...), R-tok L7).
- * dm_encode_alerts encodes the last batch of dm_process_lines (whichever kernel ran it) into `out`: one varint-length-
- * delimited DetectorSchema per anomalous record, in record order; alertID = first_alert_id + j (signed), logIDs =
- * [first_log_id + record index], detectionTimestamp = receivedTimestamp = now, extractedTimestamps = [int(float(Time))],
- * or now when the record has no Time or its Time is no float literal.  *n_alerts = anomalous records, *out_len = bytes.
+ * dm_encode_alerts encodes the last batch of dm_process_lines (whichever kernel ran it), dm_process_logs or
+ * dm_process_records into `out`: one varint-length-delimited DetectorSchema per anomalous record, in record order;
+ * alertID = first_alert_id + j (signed), detectionTimestamp = receivedTimestamp = now, extractedTimestamps =
+ * [int(float(Time))], or now when the record has no Time or its Time is no float literal.  logIDs = [first_log_id +
+ * record index] for raw lines; the record's own logID (LogSchema field 2, ParserSchema field 8, the last one; "" when
+ * absent) for the other two, which ignore first_log_id.  Time: raw lines and LogSchema texts as R-alert reads them;
+ * ParserSchema, logFormatVariables["Time"] (absent = now).  *n_alerts = anomalous records, *out_len = bytes.
  * *declined = 1 when the device cannot give the host's bytes: a Time string it cannot convert with certainty (outside
- * [0-9]{1,10}(\.[0-9]{0,6})? yet made only of bytes a float literal may hold), or an output larger than min(out_cap,
- * the out_cap of dm_set_alert_format) (*out_len then tells how large); the caller then encodes that batch on the host.
+ * [0-9]{1,10}(\.[0-9]{0,6})? yet made only of bytes a float literal may hold; for ParserSchema also any Time holding a
+ * byte >= 0x80 and no ASCII byte a float literal cannot hold), a ParserSchema batch with more anomalous records than
+ * the anomaly list holds (*out_len is then 0), or an output larger than min(out_cap, the out_cap of
+ * dm_set_alert_format) (*out_len then tells how large); the caller then encodes that batch on the host.
  * Synchronous; ends the overlap chain of dm_process_lines.  The encoder reads the batch's message, its scores and its
  * anomaly list, which the next overlapped call rewrites; so a device-resident caller must leave that call's `buf` --
  * and its `scores_out`, when it passed a device scores buffer -- unchanged until dm_encode_alerts returns, and must not
  * enqueue another dm_process_lines on the handle in between.  DM_ERR_STATE when the last batch came from another entry
- * point (dm_process_logs, dm_process_records, dm_process_values, the pipelined path). */
+ * point (dm_process_values, the pipelined path). */
 int dm_set_alert_format(dm_handle* h, uint32_t n_strings, const uint8_t* strings, const uint32_t* string_lens,
                         const uint32_t* bits_off, const uint32_t* bits, uint32_t n_combos, const uint32_t* combo_off,
                         const uint32_t* combo_members, uint32_t time_capture, uint64_t out_cap);
