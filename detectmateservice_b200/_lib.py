@@ -115,6 +115,9 @@ SYMBOLS = {
                                       C.c_uint32, C.c_uint64]),
     "dm_encode_alerts": (C.c_int, [_P, C.c_uint64, C.c_int64, C.c_int64, _P, C.c_uint64, C.POINTER(C.c_uint64),
                                    C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
+    "dm_set_parser_format": (C.c_int, [_P, C.c_uint32, C.c_char_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "dm_parse_logs": (C.c_int, [_P, _P, C.c_uint64, C.c_int, C.c_int64, C.c_int64, C.POINTER(_P), C.POINTER(C.c_uint64),
+                                C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "dm_submit_lines": (C.c_int, [_P, _P, C.c_uint64, C.c_uint64, C.c_uint32]),
     "dm_collect": (C.c_int, [_P, C.c_uint32, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "dm_collect_anomalies": (C.c_int, [_P, C.c_uint32, C.POINTER(Anomaly), C.c_uint32, C.POINTER(C.c_uint32)]),

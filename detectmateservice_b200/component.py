@@ -81,12 +81,14 @@ class Monitor:
         return f"Global - {self.label}" if self.event_id is None else f"EventID {self.event_id} - {self.label}"
 
 
-def select_component_config(config: Optional[dict], name: str, fallback: str = "NewValueDetector") -> dict:
+def select_component_config(config: Optional[dict], name: str, fallback: str = "NewValueDetector",
+                            section: str = "detectors") -> dict:
     """Pick this component's entry out of the ServiceConfig dump the loader passes
-    (src/service/core.py:127-133,144-148) and flatten ``params`` (docs/interfaces.md:74-84)."""
+    (src/service/core.py:127-133,144-148) and flatten ``params`` (docs/interfaces.md:74-84).
+    section: the top-level key holding the entries (``parsers`` for a parser)."""
     cfg = dict(config or {})
-    if isinstance(cfg.get("detectors"), dict):
-        dets = cfg["detectors"]
+    if isinstance(cfg.get(section), dict):
+        dets = cfg[section]
         pick = dets.get(name) or dets.get(fallback) or (next(iter(dets.values())) if dets else {})
         cfg = dict(pick or {})
     params = cfg.pop("params", None) or {}

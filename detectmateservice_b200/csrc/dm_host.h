@@ -40,6 +40,22 @@ inline DmFrames dm_frame_split(const uint8_t* buf, uint64_t nbytes) {
     return f;
 }
 
+// The records of a LogSchema message: the payloads of a delimited batch, or the whole message as one bare record.
+inline DmFrames dm_frame_records(const uint8_t* buf, uint64_t nbytes, bool delimited) {
+    if (delimited) return dm_frame_split(buf, nbytes);
+    DmFrames f;
+    f.off.push_back(0);
+    f.len.push_back((uint32_t)nbytes);
+    return f;
+}
+
+// A buffer that must hold `need` bytes and holds `cap`: the capacity to grow it to, or `cap` when it is large enough.
+// Grows at least twofold, so that a stream of slowly growing messages reallocates a logarithmic number of times.
+inline uint64_t dm_grow_cap(uint64_t cap, uint64_t need) {
+    if (need <= cap) return cap;
+    return std::max<uint64_t>(need, std::max<uint64_t>(2 * cap, 1u << 20));
+}
+
 // The kernels append one anomaly entry per unknown field: sorts the n entries by record and merges those of one record
 // (mask = the OR of theirs).  Returns the number of records.
 inline uint32_t dm_anomalies_merge(dm_anomaly_t* v, uint32_t n) {

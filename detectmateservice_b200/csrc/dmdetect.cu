@@ -21,6 +21,7 @@
 #include "dm_kernels_format.cuh"
 #include "dm_kernels_lanes.cuh"
 #include "dm_kernels_alerts.cuh"
+#include "dm_kernels_parse.cuh"
 #include "dm_format_host.h"
 #include "dm_host.h"
 
@@ -130,6 +131,17 @@ struct dm_handle {
     DmFormat* h_fmt = nullptr;           // host copy of the last dm_set_format[_ex] format (the encoder's is built from it)
     DmFormat* d_efmt = nullptr;          // the encoder's format: h_fmt keeping the Time capture too (dm_alert_efmt_build)
     uint32_t efmt_slots = 1;
+    // the MatcherParser stage (dm_set_parser_format / dm_parse_logs)
+    DmParseFmt* d_pf = nullptr;
+    DmFormat* d_pfmt = nullptr;          // h_fmt keeping every capture (dm_parse_efmt_build)
+    uint32_t pfmt_slots = 1;
+    bool parse_set = false;              // cleared by dm_set_format[_ex]: the parser's format is built from h_fmt
+    unsigned long long* d_psize = nullptr;   // per record its size, then the scan's tile sums and total
+    uint64_t psize_cap = 0;              // records it holds
+    uint8_t* d_pout = nullptr;           // the ParserSchemas, and their pinned host copy
+    uint8_t* h_pout = nullptr;
+    uint64_t pout_cap = 0;
+    unsigned long long* h_ptotal = nullptr;  // pinned
     // pipelined host path: two slots
     struct Slot {
         uint8_t* d_in = nullptr; uint8_t* d_flags = nullptr; float* d_scores = nullptr;
@@ -344,6 +356,8 @@ extern "C" int dm_destroy(dm_handle* h) {
     cudaFree(h->d_logs_text); cudaFree(h->d_logs); cudaFree(h->d_lhdr); cudaFreeHost(h->h_lhdr);
     cudaFree(h->d_afmt); cudaFree(h->d_ahdr); cudaFreeHost(h->h_ahdr); cudaFree(h->d_alert); cudaFree(h->d_aout);
     cudaFree(h->d_efmt); delete h->h_fmt;
+    cudaFree(h->d_pf); cudaFree(h->d_pfmt); cudaFree(h->d_psize); cudaFree(h->d_pout); cudaFreeHost(h->h_pout);
+    cudaFreeHost(h->h_ptotal);
     for (int k = 0; k < 2; ++k) {
         cudaFree(h->d_win[k]);
         if (h->ev_win_done[k]) cudaEventDestroy(h->ev_win_done[k]);
@@ -670,6 +684,7 @@ extern "C" int dm_set_format_ex(dm_handle* h, const char* log_format, const char
             h->h_fmt = f;                                        // (kept: the alert encoder's format is built from it)
             f = nullptr;
             h->fmt_norm = dm_format_norm(*h->h_fmt);
+            h->parse_set = false;
         }
     }
     delete f;
@@ -830,27 +845,22 @@ static DmLogsArgs dm_logs_args(dm_handle* h, float** scores, uint8_t** flags) {
     return a;
 }
 
-extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimited, uint32_t n_train_records,
-                               uint8_t* flags_out, float* scores_out, uint64_t out_cap,
-                               uint64_t* n_records_out, uint64_t* n_malformed_out, uint64_t* n_anomalies_out) {
-    if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
-    if (nbytes && !buf) return dm_fail(DM_ERR_ARG, "buf is NULL");
-    if (nbytes > h->max_batch_bytes) return dm_fail(DM_ERR_CAPACITY, "message of %llu bytes exceeds max_batch_bytes=%llu", (unsigned long long)nbytes, (unsigned long long)h->max_batch_bytes);
-    // framing: one bare record, or varint length, payload, varint length, payload ...
-    DmFrames fr;
-    if (delimited) {
-        fr = dm_frame_split(buf, nbytes);
-        if (fr.error) return dm_frame_fail(fr);
-    } else {
-        fr.off.push_back(0);
-        fr.len.push_back((uint32_t)nbytes);
-    }
-    const std::vector<uint32_t>& off = fr.off;
-    const std::vector<uint32_t>& len = fr.len;
-    const uint32_t n_records = (uint32_t)off.size();
+// The records of a LogSchema message (one bare record, or varint length, payload, varint length, payload ...), refused
+// where the framing is broken or they exceed max_lines.
+static int dm_logs_frames(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimited, DmFrames* fr) {
+    *fr = dm_frame_records(buf, nbytes, delimited != 0);
+    if (fr->error) return dm_frame_fail(*fr);
+    const uint32_t n_records = (uint32_t)fr->off.size();
     if (n_records > h->max_lines) return dm_fail(DM_ERR_CAPACITY, "%u records exceed max_lines=%llu", n_records, (unsigned long long)h->max_lines);
-    if ((flags_out || scores_out) && n_records > out_cap)
-        return dm_fail(DM_ERR_CAPACITY, "batch holds %u records, output capacity is %llu", n_records, (unsigned long long)out_cap);
+    return DM_OK;
+}
+
+// Enqueues the message's copy to the device and the unwrap kernels on the handle's stream, up to and including the copy
+// of the header the host reads back (h_lhdr; not synchronised).  copy: also compact the texts into d_logs_text for the
+// line path; without it the per-record text bounds and ranks are all that is computed.
+static int dm_logs_unwrap(dm_handle* h, const uint8_t* buf, uint64_t nbytes, const DmFrames& fr, uint32_t n_train_records,
+                          bool copy, DmLogsArgs* out, float** d_rscores, uint8_t** d_rflags) {
+    const uint32_t n_records = (uint32_t)fr.off.size();
     DM_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     h->last_stream = st;
@@ -861,28 +871,52 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     const uint32_t tiles = (n_records + DML_THREADS - 1) / DML_THREADS;
     int rc = dm_logs_reserve(h, n_records, n_chunks);
     if (rc != DM_OK) return rc;
-    float* d_rscores;
-    uint8_t* d_rflags;
-    DmLogsArgs a = dm_logs_args(h, &d_rscores, &d_rflags);
+    DmLogsArgs a = dm_logs_args(h, d_rscores, d_rflags);
     a.buf = h->d_in; a.n_records = n_records; a.n_train_records = n_train_records; a.per_cta = per_cta; a.n_chunks = n_chunks;
     if (nbytes) DM_CUDA(cudaMemcpyAsync(h->d_in, buf, nbytes, cudaMemcpyHostToDevice, st));
     if (n_records) {
-        DM_CUDA(cudaMemcpyAsync((void*)a.rec_off, off.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
-        DM_CUDA(cudaMemcpyAsync((void*)a.rec_len, len.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
+        DM_CUDA(cudaMemcpyAsync((void*)a.rec_off, fr.off.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
+        DM_CUDA(cudaMemcpyAsync((void*)a.rec_len, fr.len.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
         const int grid_r = (int)std::min<uint32_t>(tiles, (uint32_t)h->sm_count * 8);
-        // the copy grid covers the largest compacted size this message can have (the total is not known yet)
-        const uint64_t stores = (std::max<uint64_t>(nbytes, 1) + DML_SLACK + 15) / 16;
-        const int grid_c = (int)std::min<uint64_t>((stores + DML_THREADS - 1) / DML_THREADS, (uint64_t)h->sm_count * 16);
         dm_k_logs_walk<<<n_chunks, DML_THREADS, 0, st>>>(a);
         dm_k_logs_scan<<<1, DML_THREADS, 0, st>>>(a);
         dm_k_logs_compact<<<grid_r, DML_THREADS, 0, st>>>(a);
-        dm_k_logs_copy<<<grid_c, DML_THREADS, 0, st>>>(a);
-        h->launches += 4;
+        h->launches += 3;
+        if (copy) {
+            // the copy grid covers the largest compacted size this message can have (the total is not known yet)
+            const uint64_t stores = (std::max<uint64_t>(nbytes, 1) + DML_SLACK + 15) / 16;
+            const int grid_c = (int)std::min<uint64_t>((stores + DML_THREADS - 1) / DML_THREADS, (uint64_t)h->sm_count * 16);
+            dm_k_logs_copy<<<grid_c, DML_THREADS, 0, st>>>(a);
+            h->launches++;
+        }
         DM_CUDA(cudaGetLastError());
     } else {
         DM_CUDA(cudaMemsetAsync(h->d_lhdr, 0, sizeof(DmLogsHeader), st));
     }
     DM_CUDA(cudaMemcpyAsync(h->h_lhdr, h->d_lhdr, sizeof(DmLogsHeader), cudaMemcpyDeviceToHost, st));
+    *out = a;
+    return DM_OK;
+}
+
+extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimited, uint32_t n_train_records,
+                               uint8_t* flags_out, float* scores_out, uint64_t out_cap,
+                               uint64_t* n_records_out, uint64_t* n_malformed_out, uint64_t* n_anomalies_out) {
+    if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
+    if (nbytes && !buf) return dm_fail(DM_ERR_ARG, "buf is NULL");
+    if (nbytes > h->max_batch_bytes) return dm_fail(DM_ERR_CAPACITY, "message of %llu bytes exceeds max_batch_bytes=%llu", (unsigned long long)nbytes, (unsigned long long)h->max_batch_bytes);
+    DmFrames fr;
+    int rc = dm_logs_frames(h, buf, nbytes, delimited, &fr);
+    if (rc != DM_OK) return rc;
+    const uint32_t n_records = (uint32_t)fr.off.size();
+    if ((flags_out || scores_out) && n_records > out_cap)
+        return dm_fail(DM_ERR_CAPACITY, "batch holds %u records, output capacity is %llu", n_records, (unsigned long long)out_cap);
+    DmLogsArgs a;
+    float* d_rscores;
+    uint8_t* d_rflags;
+    rc = dm_logs_unwrap(h, buf, nbytes, fr, n_train_records, true, &a, &d_rscores, &d_rflags);
+    if (rc != DM_OK) return rc;
+    cudaStream_t st = h->stream;
+    const uint32_t tiles = (n_records + DML_THREADS - 1) / DML_THREADS;
     DM_CUDA(cudaStreamSynchronize(st));
     const DmLogsHeader lh = *h->h_lhdr;
     if (lh.n_lines) {
@@ -1080,6 +1114,114 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
 // ---------------------------------------------------------------------------------------
 // pipelined host path
 // ---------------------------------------------------------------------------------------
+// ---------------------------------------------------------------------------------------
+// The MatcherParser stage: LogSchema records in, ParserSchemas out (dm_kernels_parse.cuh)
+// ---------------------------------------------------------------------------------------
+extern "C" int dm_set_parser_format(dm_handle* h, uint32_t n_strings, const uint8_t* strings, const uint32_t* string_lens,
+                                    const uint32_t* capture_order) {
+    if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
+    if (!h->fmt_set || !h->h_fmt) return dm_fail(DM_ERR_STATE, "dm_set_format has not been called");
+    if (!string_lens || (!strings && n_strings)) return dm_fail(DM_ERR_ARG, "strings missing");
+    DmParseFmt* P = new (std::nothrow) DmParseFmt;
+    DmFormat* pf = new (std::nothrow) DmFormat;
+    if (!P || !pf) { delete P; delete pf; return dm_fail(DM_ERR_ARG, "out of host memory"); }
+    const char* why = dm_parse_fmt_build(*h->h_fmt, n_strings, strings, string_lens, capture_order, P);
+    if (why) { delete P; delete pf; return dm_fail(DM_ERR_ARG, "dm_set_parser_format: %s", why); }
+    dm_parse_efmt_build(*h->h_fmt, pf);
+    cudaError_t e = cudaSetDevice(h->device);
+    if (e == cudaSuccess && !h->d_pf) e = cudaMalloc(&h->d_pf, sizeof(DmParseFmt));
+    if (e == cudaSuccess && !h->d_pfmt) e = cudaMalloc(&h->d_pfmt, sizeof(DmFormat));
+    if (e == cudaSuccess && !h->h_ptotal) e = cudaHostAlloc(&h->h_ptotal, sizeof(unsigned long long), cudaHostAllocDefault);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->last_stream);
+    if (e == cudaSuccess) e = cudaMemcpy(h->d_pf, P, sizeof(DmParseFmt), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(h->d_pfmt, pf, sizeof(DmFormat), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) h->pfmt_slots = pf->max_slots;
+    delete P;
+    delete pf;
+    if (e != cudaSuccess) return dm_fail(DM_ERR_CUDA, "dm_set_parser_format: %s", cudaGetErrorString(e));
+    h->parse_set = true;
+    return DM_OK;
+}
+
+extern "C" int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimited, int64_t first_parsed_id,
+                             int64_t now, const uint8_t** out, uint64_t* out_len, uint64_t* n_records_out,
+                             uint64_t* n_emitted_out, uint64_t* n_malformed_out) {
+    if (!h || !out || !out_len) return dm_fail(DM_ERR_ARG, "NULL argument");
+    if (nbytes && !buf) return dm_fail(DM_ERR_ARG, "buf is NULL");
+    if (!h->parse_set) return dm_fail(DM_ERR_STATE, "dm_set_parser_format has not been called since the last dm_set_format");
+    if (nbytes > h->max_batch_bytes) return dm_fail(DM_ERR_CAPACITY, "message of %llu bytes exceeds max_batch_bytes=%llu", (unsigned long long)nbytes, (unsigned long long)h->max_batch_bytes);
+    *out = h->h_pout;
+    *out_len = 0;
+    DmFrames fr;
+    int rc = dm_logs_frames(h, buf, nbytes, delimited, &fr);
+    if (rc != DM_OK) return rc;
+    const uint32_t n_records = (uint32_t)fr.off.size();
+    h->last_src = DM_SRC_NONE;                                // (d_in no longer holds the last detected batch)
+    DmLogsArgs la;
+    float* rscores;
+    uint8_t* rflags;
+    rc = dm_logs_unwrap(h, buf, nbytes, fr, 0, false, &la, &rscores, &rflags);
+    if (rc != DM_OK) return rc;
+    cudaStream_t st = h->stream;
+    const uint64_t tiles = dm_alert_tiles(n_records) + 1;
+    if (n_records + tiles + 1 > h->psize_cap) {
+        DM_CUDA(cudaStreamSynchronize(st));
+        cudaFree(h->d_psize);
+        h->d_psize = nullptr;
+        h->psize_cap = 0;
+        const uint64_t cap = std::max<uint64_t>(2 * (n_records + tiles + 1), 8192);
+        DM_CUDA(cudaMalloc(&h->d_psize, cap * sizeof(unsigned long long)));
+        h->psize_cap = cap;
+    }
+    DmParseArgs a;
+    a.pf = h->d_pf; a.pfmt = h->d_pfmt; a.buf = h->d_in; a.nbuf = h->d_norm; a.n_records = n_records;
+    a.rec_off = la.rec_off; a.rec_len = la.rec_len; a.text_off = la.text_off; a.text_len = la.text_len; a.rank = la.rec_line;
+    a.size = h->d_psize; a.first_id = first_parsed_id; a.now = now;
+    unsigned long long* tile_sums = h->d_psize + n_records;
+    unsigned long long* d_total = tile_sums + tiles;
+    a.total = d_total;
+    const bool norm = h->fmt_norm;
+    if (norm && !h->d_norm) return dm_fail(DM_ERR_STATE, "no R-norm scratch");
+    const size_t smem = (size_t)2 * h->pfmt_slots * DM_FMTL_THREADS * sizeof(uint2);
+    const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>((n_records + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS, (uint32_t)h->sm_count * 32));
+    DM_CUDA(cudaMemsetAsync(d_total, 0, sizeof(unsigned long long), st));
+    if (n_records) {
+        dm_parse_kernel(norm, false)<<<grid, DM_FMTL_THREADS, smem, st>>>(a);
+        dm_alert_scan<unsigned long long>(a.size, n_records, tile_sums, d_total, st);
+        h->launches += 4;
+        DM_CUDA(cudaGetLastError());
+    }
+    DM_CUDA(cudaMemcpyAsync(h->h_ptotal, d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
+    const uint64_t total = *h->h_ptotal, n_emitted = h->h_lhdr->n_lines;
+    const uint64_t cap = dm_grow_cap(h->pout_cap, total);
+    if (cap != h->pout_cap) {
+        cudaFree(h->d_pout);
+        cudaFreeHost(h->h_pout);
+        h->d_pout = nullptr;
+        h->h_pout = nullptr;
+        h->pout_cap = 0;
+        *out = nullptr;
+        DM_CUDA(cudaMalloc(&h->d_pout, cap));
+        DM_CUDA(cudaHostAlloc(&h->h_pout, cap, cudaHostAllocDefault));
+        h->pout_cap = cap;
+    }
+    if (total) {
+        a.out = h->d_pout; a.out_cap = h->pout_cap;
+        dm_parse_kernel(norm, true)<<<grid, DM_FMTL_THREADS, smem, st>>>(a);
+        h->launches++;
+        DM_CUDA(cudaGetLastError());
+        DM_CUDA(cudaMemcpyAsync(h->h_pout, h->d_pout, total, cudaMemcpyDeviceToHost, st));
+        DM_CUDA(cudaStreamSynchronize(st));
+    }
+    *out = h->h_pout;
+    *out_len = total;
+    if (n_records_out) *n_records_out = n_records;
+    if (n_emitted_out) *n_emitted_out = n_emitted;
+    if (n_malformed_out) *n_malformed_out = n_records - n_emitted;
+    return DM_OK;
+}
+
 static int dm_slots_init(dm_handle* h) {
     if (h->slots_ready) return DM_OK;
     DM_CUDA(cudaStreamCreateWithFlags(&h->st_in, cudaStreamNonBlocking));

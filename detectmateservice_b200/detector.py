@@ -20,6 +20,15 @@ def _as_key_bytes(k: Union[str, bytes]) -> bytes:
     return k if isinstance(k, bytes) else k.encode("utf-8")
 
 
+def parser_format_strings(version: str, parser_type: str, parser_id: str, templates: Sequence[bytes],
+                          names: Sequence[str]) -> Tuple[List[bytes], List[int]]:
+    """dm_set_parser_format's strings and capture_order: the capture names go out sorted by their UTF-8 bytes, as
+    wire.encode_parser_schema sorts the logFormatVariables keys."""
+    order = sorted(range(len(names)), key=lambda i: names[i].encode("utf-8"))
+    strs = [s.encode("utf-8") for s in (version, parser_type, parser_id)] + [bytes(t) for t in templates]
+    return strs + [names[i].encode("utf-8") for i in order], order
+
+
 class DeviceDetector:
     """NewValueDetector state (known-value table + running statistics) on one H100.
 
@@ -308,6 +317,30 @@ class DeviceDetector:
         if declined.value:
             return None
         return bytes(buf.numpy()[:out_len.value]), int(n.value)
+
+    # ------------------------------------------------------------------ the MatcherParser stage on the device
+    def set_parser_format(self, version: str, parser_type: str, parser_id: str, templates: Sequence[bytes],
+                          names: Sequence[str]) -> None:
+        """What parse_logs() writes besides the record's own text (dm_set_parser_format), after set_format(): the
+        constant strings, the template texts verbatim in EventID order and the log_format's capture names in capture
+        order (written sorted by their UTF-8 bytes)."""
+        strs, order = parser_format_strings(version, parser_type, parser_id, templates, names)
+        lens = (C.c_uint32 * len(strs))(*[len(s) for s in strs])
+        _lib.check(self._lib.dm_set_parser_format(self._h, len(strs), b"".join(strs), lens,
+                                                  (C.c_uint32 * max(1, len(order)))(*order)))
+
+    def parse_logs(self, buf: BytesLike, delimited: bool, first_parsed_id: int, now: int) -> Tuple[bytes, int, int, int]:
+        """LogSchema records -- one bare record (delimited=False) or a varint-length-delimited batch -- parsed on the
+        device into ParserSchemas (dm_parse_logs, rule R-parse in DESIGN.md).  Returns (the varint-delimited
+        ParserSchemas, records, ParserSchemas emitted, records malformed or unusable)."""
+        ptr, n, keep = self._host_ptr(buf)
+        out, out_len = C.c_void_p(), C.c_uint64()
+        n_rec, n_emit, n_bad = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        _lib.check(self._lib.dm_parse_logs(self._h, ptr, n, int(bool(delimited)), int(first_parsed_id), int(now),
+                                           C.byref(out), C.byref(out_len), C.byref(n_rec), C.byref(n_emit), C.byref(n_bad)))
+        del keep
+        blob = C.string_at(out.value, out_len.value) if out_len.value else b""
+        return blob, n_rec.value, n_emit.value, n_bad.value
 
     def sync(self) -> Tuple[int, int]:
         n_lines = C.c_uint64()

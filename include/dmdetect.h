@@ -286,6 +286,29 @@ int dm_set_alert_format(dm_handle* h, uint32_t n_strings, const uint8_t* strings
 int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t first_alert_id, int64_t now, uint8_t* out,
                      uint64_t out_cap, uint64_t* out_len, uint64_t* n_alerts, int* declined);
 
+/* The MatcherParser stage on the device (rule R-parse, DESIGN.md): LogSchema records in, ParserSchema records out,
+ * the bytes the parser component's host path writes (parser.py, wire.encode_parser_schema).  The detector's known set
+ * is not touched: a handle with n_keys = 0 (dm_set_monitors with no monitors) and the smallest table is enough.
+ * dm_set_parser_format, after dm_set_format[_ex] (and again after every later dm_set_format[_ex]): n_strings strings,
+ * concatenated: __version__, parserType, parserID, the template texts verbatim in EventID order, then the names of the
+ * log_format's captures in output order (sorted by their UTF-8 bytes); name j is capture capture_order[j].
+ * dm_parse_logs takes one bare LogSchema record (delimited = 0) or a varint-length-delimited batch, framed and checked
+ * as dm_process_logs (R-log).  A malformed or unusable record gives no output; every other one gives one ParserSchema:
+ *   EventID    the template the Content matched (-1: none, or the log_format did not match)
+ *   template   that template's text (EventID >= 0 only); variables: its wildcards (slices of the R-norm Content)
+ *   parsedLogID  first_parsed_id + the number of records emitted before it in this call, in decimal
+ *   logID      the record's last field 2 ("" when absent); log: its text
+ *   logFormatVariables  every capture of the log_format, when it matched
+ *   receivedTimestamp = parsedTimestamp = now
+ * *out = the varint-length-delimited ParserSchemas in record order, *out_len bytes, in a pinned buffer the handle owns,
+ * valid until the next dm_parse_logs.  *n_emitted = ParserSchemas, *n_malformed = malformed + unusable records.
+ * Synchronous; ends the overlap chain of dm_process_lines, and dm_encode_alerts no longer has a batch to encode. */
+int dm_set_parser_format(dm_handle* h, uint32_t n_strings, const uint8_t* strings, const uint32_t* string_lens,
+                         const uint32_t* capture_order);
+int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimited, int64_t first_parsed_id, int64_t now,
+                  const uint8_t** out, uint64_t* out_len, uint64_t* n_records_out, uint64_t* n_emitted_out,
+                  uint64_t* n_malformed_out);
+
 /* Pipelined host path (two slots): dm_submit_lines enqueues, without waiting, the copy of a
  * HOST message (pinned memory gives real overlap) to the device, the kernels and the copy
  * of the batch header back; dm_collect waits for that slot, copies the slot's flags and
