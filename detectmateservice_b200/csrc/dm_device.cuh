@@ -215,14 +215,19 @@ static inline DmDetectArgs dm_detect_args(const uint8_t* buf, uint64_t nbytes, c
     return a;
 }
 
+// The grid of a grid-stride kernel over n items, `threads` per CTA: one item per thread, capped at max_grid CTAs, at
+// least one CTA.
+static inline unsigned dm_grid(uint64_t n, unsigned threads, uint64_t max_grid) {
+    const uint64_t want = (n + threads - 1) / threads;
+    const uint64_t grid = want < max_grid ? want : max_grid;
+    return (unsigned)(grid > 1 ? grid : 1);
+}
+
 // Their grid.  The number of records is only known on the device: the grid is sized for the most the message can hold
 // (one per byte pair, at most max_lines), capped at max_grid CTAs (the kernels stride); CTAs past the last record leave
 // after one compare.
 static inline unsigned dm_detect_grid(uint64_t nbytes, uint64_t max_lines, unsigned threads, uint64_t max_grid) {
-    const uint64_t max_recs = nbytes / 2 + 1 < max_lines ? nbytes / 2 + 1 : max_lines;
-    const uint64_t want = (max_recs + threads - 1) / threads;
-    const uint64_t grid = want < max_grid ? want : max_grid;
-    return (unsigned)(grid > 1 ? grid : 1);
+    return dm_grid(nbytes / 2 + 1 < max_lines ? nbytes / 2 + 1 : max_lines, threads, max_grid);
 }
 
 // ---------------------------------------------------------------------------------------

@@ -12,7 +12,7 @@
 //                       a record the device cannot word exactly (its Time string is outside the grammar) declines
 //   dm_alert_scan       exclusive scan of the sizes: where each DetectorSchema goes; the total
 //   dm_k_alert_write    one thread per anomalous record: the same walk as dm_k_alert_size, writing
-// In log_format mode dm_k_alert_format<NORM, false / true> takes the place of the size / write kernels: it re-runs the
+// In log_format mode dm_k_alert_format (NORM, !WRITE / WRITE) takes the place of the size / write kernels: it re-runs the
 // header and template chains with the matcher's own device functions (dm_fmtl_*, dm_kernels_format.cuh) before the walk.
 // LogSchema batches (DMA_LOGS) take the same launches: dm_k_logs_scatter has already rewritten the anomaly list to
 // record indices, and a record's text is its line of the compacted buffer, so only dm_k_alert_gather (where the text
@@ -34,6 +34,7 @@
 #define DMA_LINES 0u                               // DmAlertArgs::src: the batch came from dm_process_lines,
 #define DMA_LOGS 1u                                //   dm_process_logs
 #define DMA_RECORDS 2u                             //   or dm_process_records
+#define DMA_SRC_NONE 0xFFu                         //   or none of them: there is nothing to word
 
 // What dm_set_alert_format fixes: everything of a DetectorSchema that does not depend on the record or the call.
 struct DmAlertFmt {
@@ -688,6 +689,69 @@ static inline void dm_alert_efmt_build(const DmFormat& f, uint32_t time_cap, DmF
 }
 
 // ---------------------------------------------------------------------------------------------- host side
+// Plain C++ from here on, shared by libdmdetect and the CPU emulator of tests/.
+//
+// The tiles of a scan over n elements.
+static inline uint64_t dm_alert_tiles(uint64_t n) { return (n + DMA_TILE - 1) / DMA_TILE; }
+
+// The encoder's scratch for max_lines records and an anomaly list of anomaly_cap entries, one block: per record + 1
+// its rank (u32); per entry + 1 its offset and size (u64); the scans' tile sums (u64); per entry + 1 its record and
+// merged mask (u32).  Carves the block at base into a's arrays and *tile_sums (base nullptr: only sizes it); returns
+// its size in bytes.
+static inline uint64_t dm_alert_scratch(uint8_t* base, uint64_t max_lines, uint32_t anomaly_cap, DmAlertArgs* a,
+                                        unsigned long long** tile_sums) {
+    const uint64_t lines = max_lines + 1, recs = (uint64_t)anomaly_cap + 1;
+    const uint64_t off = (4 * lines + 7) & ~7ull, size = off + 8 * recs, tiles = size + 8 * recs;
+    const uint64_t line = tiles + 8 * (dm_alert_tiles(lines > recs ? lines : recs) + 1), mask = line + 4 * recs;
+    if (base) {
+        a->rank = (uint32_t*)base;
+        a->rec_off = (unsigned long long*)(base + off);
+        a->size = (unsigned long long*)(base + size);
+        *tile_sums = (unsigned long long*)(base + tiles);
+        a->rec_line = (uint32_t*)(base + line);
+        a->rec_mask = (uint32_t*)(base + mask);
+    }
+    return mask + 4 * recs;
+}
+
+// What the encoder takes from the last batch of source src (DMA_*): *n_lines records (ParserSchema: n_records, the
+// others: the header's) and the anomaly entries it returns (ParserSchema: the flagged records, the others: the list's,
+// at most its capacity).  0: nothing to word.  *declined: the batch declines before any launch, having more anomalous
+// records than the per-record arrays hold (the return value is then their count).
+static inline uint64_t dm_alert_entries(uint32_t src, const DmBatchHeader& hdr, uint64_t n_records, uint32_t anomaly_cap,
+                                        uint64_t* n_lines, bool* declined) {
+    const bool records = src == DMA_RECORDS;
+    *n_lines = records ? n_records : hdr.n_lines;
+    const uint64_t n = records ? hdr.n_anomalies : (hdr.anomaly_list_count < anomaly_cap ? hdr.anomaly_list_count : anomaly_cap);
+    *declined = false;
+    if (n == 0 || *n_lines == 0) return 0;
+    *declined = n > anomaly_cap;
+    return n;
+}
+
+// The instantiations the encoder runs.
+typedef void (*DmAlertKernel)(DmAlertArgs);
+
+// Marking the anomalous records (!gather) and gathering their masks: one thread per anomaly entry, or for ParserSchema
+// batches one per record (*items: what the threads stride over).
+static inline DmAlertKernel dm_alert_mark_kernel(uint32_t src, bool gather, uint64_t n_lines, uint64_t entries,
+                                                 uint64_t* items) {
+    *items = src == DMA_RECORDS ? n_lines : entries;
+    if (src == DMA_RECORDS) return gather ? dm_k_alert_gather_records : dm_k_alert_mark_records;
+    return gather ? dm_k_alert_gather : dm_k_alert_mark;
+}
+
+// The size (!write) and the write pass, one thread per anomalous record.  fmt: the batch was detected in log_format
+// mode, norm: with R-norm.  *fmtl: the pass is dm_k_alert_format, which runs DM_FMTL_THREADS per CTA with the
+// captures in dynamic shared memory (the others run DMA_THREADS per CTA).
+static inline DmAlertKernel dm_alert_pass_kernel(uint32_t src, bool fmt, bool norm, bool write, bool* fmtl) {
+    *fmtl = src != DMA_RECORDS && fmt;
+    if (src == DMA_RECORDS) return write ? dm_k_alert_records<true> : dm_k_alert_records<false>;
+    if (!fmt) return write ? dm_k_alert_write : dm_k_alert_size;
+    if (norm) return write ? dm_k_alert_format<true, true> : dm_k_alert_format<true, false>;
+    return write ? dm_k_alert_format<false, true> : dm_k_alert_format<false, false>;
+}
+
 // Fills f from the handle's keys and dm_set_alert_format's arguments.  strings = version, detectorID, detectorType,
 // description, then the n_strings - 4 alert keys in output order; alert key j is supplied by the mask bits
 // bits[bits_off[j], bits_off[j + 1]).  Returns nullptr or the reason the arguments are refused.

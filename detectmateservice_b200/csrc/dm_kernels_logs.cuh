@@ -68,6 +68,63 @@ static inline uint32_t dm_logs_plan(uint32_t n_records, uint32_t max_ctas, uint3
     return (n_records + *per_cta - 1) / *per_cta;
 }
 
+// The host side of the unwrap: plain C++, shared by libdmdetect and the CPU emulator of tests/.
+//
+// The per-record and per-chunk arrays for up to `cap` records and `chunks` walk chunks, one block: loc and chunk (u64),
+// the eight u32 arrays of DmLogsArgs (cap + 1 each), then per record a score (f32) and a flag (u8), dm_k_logs_scatter's
+// outputs.  Its size in bytes.
+static inline uint64_t dm_logs_scratch_bytes(uint64_t cap, uint32_t chunks) {
+    return 8 * (cap + chunks) + 4 * 8 * (cap + 1) + 4 * cap + cap + 16;
+}
+
+// That block at base, carved into the arrays of a DmLogsArgs (header lhdr) and the per-record *scores and *flags.
+static inline DmLogsArgs dm_logs_carve(void* base, uint64_t cap, uint32_t chunks, DmLogsHeader* lhdr, float** scores,
+                                       uint8_t** flags) {
+    DmLogsArgs a{};
+    unsigned long long* w = (unsigned long long*)base;
+    a.loc = w;
+    a.chunk = w + cap;
+    uint32_t* u = (uint32_t*)(w + cap + chunks);
+    uint32_t* arr[8];
+    for (int i = 0; i < 8; ++i) arr[i] = u + (uint64_t)i * (cap + 1);
+    a.rec_off = arr[0]; a.rec_len = arr[1]; a.text_off = arr[2]; a.text_len = arr[3];
+    a.rec_line = arr[4]; a.line_src = arr[5]; a.line_dst = arr[6]; a.line_rec = arr[7];
+    *scores = (float*)(u + 8 * (cap + 1));
+    *flags = (uint8_t*)(*scores + cap);
+    a.lhdr = lhdr;
+    return a;
+}
+
+// The fields of one call: the message, its records, and the walk's plan on at most walk_ctas CTAs.  out: the buffer
+// dm_k_logs_copy compacts the texts into (nullptr when the call does not copy them).
+static inline void dm_logs_call(DmLogsArgs* a, const uint8_t* buf, uint32_t n_records, uint32_t n_train_records,
+                                uint32_t walk_ctas, uint8_t* out, uint64_t out_cap) {
+    a->buf = buf;
+    a->n_records = n_records;
+    a->n_train_records = n_train_records;
+    a->n_chunks = dm_logs_plan(n_records, walk_ctas, &a->per_cta);
+    a->out = out;
+    a->out_cap = out_cap;
+}
+
+// The compacted texts of a message of up to max_bytes bytes need at most max_bytes + 1 bytes, whatever the message:
+// every record spends at least len + 1 bytes of it on a text of len bytes -- the text plus its length prefix, or (a
+// bare record) plus the `log` field's tag and length -- except a bare record of zero bytes, which compacts to a single
+// '\n'.  The slack the line kernels read past the end, and the rounding to whole 16-byte stores, come on top.
+static inline uint64_t dm_logs_text_bytes(uint64_t max_bytes) { return (max_bytes + 1 + DML_SLACK + 15) & ~15ull; }
+
+// dm_k_logs_copy's grid: one 16-byte store per thread over the largest compacted size a message of nbytes bytes can
+// have (the total is not known before the launch).
+static inline unsigned dm_logs_copy_grid(uint64_t nbytes, uint64_t max_ctas) {
+    return dm_grid(((nbytes ? nbytes : 1) + DML_SLACK + 15) / 16, DML_THREADS, max_ctas);
+}
+
+// dm_k_logs_scatter's grid: a thread per record, and at least the whole CTAs of the anomaly list's capacity.
+static inline unsigned dm_logs_scatter_grid(uint32_t n_records, uint32_t anomaly_cap, uint64_t max_ctas) {
+    const uint64_t list = (uint64_t)anomaly_cap / DML_THREADS * DML_THREADS;
+    return dm_grid(n_records > list ? n_records : list, DML_THREADS, max_ctas);
+}
+
 // Walks one LogSchema record [pos, end).  False where protobuf's runtime refuses the record, and for a group; else
 // [tp, tp + tl) is the last `log` field (tl = 0 when there is none).  A field 1-5 under another wire type is an
 // unknown field to protobuf and skipped; an unknown LEN field is not checked for UTF-8.

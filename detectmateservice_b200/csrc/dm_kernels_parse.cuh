@@ -18,6 +18,7 @@
 #include "dm_device.cuh"
 #include "dm_kernels_logs.cuh"
 #include "dm_kernels_format.cuh"
+#include "dm_kernels_alerts.cuh"
 
 #define DMP_POOL 65536                             // bytes of constant text: fields 1-3, template texts, capture names
 
@@ -235,6 +236,31 @@ static inline DmParseKernel dm_parse_kernel(bool norm, bool write) {
 }
 
 // ---------------------------------------------------------------------------------------------- host side
+// The arguments of both passes over the records the unwrap (la) walked: their payloads, texts and ranks.  out / out_cap
+// are set before the write pass.
+static inline DmParseArgs dm_parse_args(const DmLogsArgs& la, const DmParseFmt* pf, const DmFormat* pfmt, uint8_t* nbuf,
+                                        long long first_id, long long now) {
+    DmParseArgs a{};
+    a.pf = pf; a.pfmt = pfmt; a.buf = la.buf; a.nbuf = nbuf; a.n_records = la.n_records;
+    a.rec_off = la.rec_off; a.rec_len = la.rec_len; a.text_off = la.text_off; a.text_len = la.text_len; a.rank = la.rec_line;
+    a.first_id = first_id; a.now = now;
+    return a;
+}
+
+// The size pass's scratch for n_records records, one block of u64: per record its size (a->size), the scan's tile sums
+// (*tile_sums), the total (a->total, *total).  Carves the block at base (nullptr: only sizes it); returns its words.
+static inline uint64_t dm_parse_scratch(unsigned long long* base, uint32_t n_records, DmParseArgs* a,
+                                        unsigned long long** tile_sums, unsigned long long** total) {
+    const uint64_t tiles = dm_alert_tiles(n_records) + 1;
+    if (base) {
+        a->size = base;
+        *tile_sums = base + n_records;
+        *total = base + n_records + tiles;
+        a->total = *total;
+    }
+    return n_records + tiles + 1;
+}
+
 // The matcher's format as the parser needs it: chain 0 keeps every capture and every template every wildcard, so that
 // capture c and variable v sit in slot c and v.
 static inline void dm_parse_efmt_build(const DmFormat& f, DmFormat* out) {

@@ -58,9 +58,6 @@ extern "C" uint64_t dm_table_key(uint32_t field, const uint8_t* value, uint32_t 
 // ---------------------------------------------------------------------------------------
 // handle
 // ---------------------------------------------------------------------------------------
-// Where the last batch came from (dm_handle::last_src): the batches dm_encode_alerts can word, or none of them.
-enum { DM_SRC_NONE = 0, DM_SRC_LINES, DM_SRC_LOGS, DM_SRC_RECORDS };
-
 struct dm_handle {
     int device = 0;
     int sm_count = 0;
@@ -119,7 +116,7 @@ struct dm_handle {
     // DetectorSchema alerts on the device (dm_set_alert_format / dm_encode_alerts), allocated by dm_set_alert_format
     const uint8_t* last_buf = nullptr;   // the last dm_process_lines batch as its kernels read it, and its scores
     const float* last_scores = nullptr;
-    uint32_t last_src = DM_SRC_NONE;     // where the last batch came from: what dm_encode_alerts can word
+    uint32_t last_src = DMA_SRC_NONE;    // where the last batch came from: what dm_encode_alerts can word
     uint32_t last_n_records = 0;         // its records (dm_process_records)
     DmAlertFmt* d_afmt = nullptr;
     DmAlertHeader* d_ahdr = nullptr;
@@ -486,7 +483,7 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     if (!stream_kernel) h->dmx.chain_stream = nullptr;     // (a launch that is not the stream kernel's ends the overlap chain)
     h->last_buf = d_buf;
     h->last_scores = d_scores;
-    h->last_src = DM_SRC_LINES;
+    h->last_src = DMA_LINES;
 
     const bool want_sync = host_out || n_lines_out || n_anomalies_out;
     if (!want_sync) return DM_OK;
@@ -541,7 +538,7 @@ extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blo
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
-    h->last_src = DM_SRC_NONE;
+    h->last_src = DMA_SRC_NONE;
     if (n_values > h->vals_cap) {
         if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
         h->vals_cap = std::max<uint64_t>(2ull * n_values, 4096);
@@ -739,7 +736,7 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     cudaStream_t st = h->stream;
     h->last_stream = st;
     dm_break_chain(h, st);
-    h->last_src = DM_SRC_NONE;
+    h->last_src = DMA_SRC_NONE;
     if (2ull * n_records + 2 > 3ull * h->vals_cap + 1) {
         if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
         h->vals_cap = std::max<uint64_t>(2ull * n_records, 4096);
@@ -792,7 +789,7 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     if (rc != DM_OK) return rc;
     if (n_records_out) *n_records_out = n_records;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
-    h->last_src = DM_SRC_RECORDS;
+    h->last_src = DMA_RECORDS;
     h->last_n_records = n_records;
     return DM_OK;
 }
@@ -800,49 +797,25 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
 // ---------------------------------------------------------------------------------------
 // LogSchema input (the reader stage's records): unwrapped on the device, then the line path
 // ---------------------------------------------------------------------------------------
-// The compacted texts need at most max_batch_bytes + 1 bytes, whatever the batch: every record spends at least len + 1
-// bytes of the caller's message on a text of len bytes -- the text plus its length prefix, or (a bare record) plus
-// the `log` field's tag and length -- except a bare record of zero bytes, which compacts to a single '\n'.  The slack
-// the line kernels read past the end, and the rounding to whole 16-byte stores, come on top.  So one buffer, allocated
-// on the first call, serves every call.  The per-record arrays grow with the largest batch seen.
-static int dm_logs_reserve(dm_handle* h, uint64_t n_records, uint32_t n_chunks) {
+// The compacted texts (dm_logs_text_bytes): one buffer, allocated on the first call, serves every call.  The
+// per-record arrays (dm_logs_scratch_bytes) grow with the largest batch seen; they hold `chunks` walk chunks, the most
+// any of the handle's walk plans makes.
+static int dm_logs_reserve(dm_handle* h, uint64_t n_records, uint32_t chunks) {
     if (!h->d_lhdr) {
         DM_CUDA(cudaMalloc(&h->d_lhdr, sizeof(DmLogsHeader)));
         DM_CUDA(cudaHostAlloc(&h->h_lhdr, sizeof(DmLogsHeader), cudaHostAllocDefault));
-        h->logs_text_cap = (h->max_batch_bytes + 1 + DML_SLACK + 15) & ~15ull;
+        h->logs_text_cap = dm_logs_text_bytes(h->max_batch_bytes);
         DM_CUDA(cudaMalloc(&h->d_logs_text, h->logs_text_cap));
     }
-    if (n_records <= h->logs_cap && n_chunks <= h->logs_chunks) return DM_OK;
+    if (n_records <= h->logs_cap) return DM_OK;
     const uint64_t cap = std::min<uint64_t>(std::max<uint64_t>({n_records, 2 * h->logs_cap, 4096}), h->max_lines);
-    const uint32_t chunks = std::max<uint32_t>(n_chunks, (uint32_t)h->sm_count * 4);
     if (h->d_logs) DM_CUDA(cudaFree(h->d_logs));
     h->d_logs = nullptr;
     h->logs_cap = 0;
-    // loc + chunk (u64), 8 u32 arrays of cap + 1, scores (f32), flags (u8)
-    DM_CUDA(cudaMalloc(&h->d_logs, 8 * (cap + chunks) + 4 * 8 * (cap + 1) + 4 * cap + cap + 16));
+    DM_CUDA(cudaMalloc(&h->d_logs, dm_logs_scratch_bytes(cap, chunks)));
     h->logs_cap = cap;
     h->logs_chunks = chunks;
     return DM_OK;
-}
-
-// The arrays of dm_logs_reserve, carved out of one allocation.
-static DmLogsArgs dm_logs_args(dm_handle* h, float** scores, uint8_t** flags) {
-    DmLogsArgs a;
-    const uint64_t cap = h->logs_cap;
-    unsigned long long* w = (unsigned long long*)h->d_logs;
-    a.loc = w;
-    a.chunk = w + cap;
-    uint32_t* u = (uint32_t*)(w + cap + h->logs_chunks);
-    uint32_t* arr[8];
-    for (int i = 0; i < 8; ++i) arr[i] = u + (uint64_t)i * (cap + 1);
-    a.rec_off = arr[0]; a.rec_len = arr[1]; a.text_off = arr[2]; a.text_len = arr[3];
-    a.rec_line = arr[4]; a.line_src = arr[5]; a.line_dst = arr[6]; a.line_rec = arr[7];
-    *scores = (float*)(u + 8 * (cap + 1));
-    *flags = (uint8_t*)(*scores + cap);
-    a.out = h->d_logs_text;
-    a.out_cap = h->logs_text_cap;
-    a.lhdr = h->d_lhdr;
-    return a;
 }
 
 // The records of a LogSchema message (one bare record, or varint length, payload, varint length, payload ...), refused
@@ -866,27 +839,22 @@ static int dm_logs_unwrap(dm_handle* h, const uint8_t* buf, uint64_t nbytes, con
     h->last_stream = st;
     dm_break_chain(h, st);
     // walk grid: at most 4 CTAs per SM
-    uint32_t per_cta;
-    const uint32_t n_chunks = dm_logs_plan(n_records, (uint32_t)h->sm_count * 4, &per_cta);
-    const uint32_t tiles = (n_records + DML_THREADS - 1) / DML_THREADS;
-    int rc = dm_logs_reserve(h, n_records, n_chunks);
+    const uint32_t walk_ctas = (uint32_t)h->sm_count * 4;
+    int rc = dm_logs_reserve(h, n_records, walk_ctas);
     if (rc != DM_OK) return rc;
-    DmLogsArgs a = dm_logs_args(h, d_rscores, d_rflags);
-    a.buf = h->d_in; a.n_records = n_records; a.n_train_records = n_train_records; a.per_cta = per_cta; a.n_chunks = n_chunks;
+    DmLogsArgs a = dm_logs_carve(h->d_logs, h->logs_cap, h->logs_chunks, h->d_lhdr, d_rscores, d_rflags);
+    dm_logs_call(&a, h->d_in, n_records, n_train_records, walk_ctas, copy ? h->d_logs_text : nullptr,
+                 copy ? h->logs_text_cap : 0);
     if (nbytes) DM_CUDA(cudaMemcpyAsync(h->d_in, buf, nbytes, cudaMemcpyHostToDevice, st));
     if (n_records) {
         DM_CUDA(cudaMemcpyAsync((void*)a.rec_off, fr.off.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync((void*)a.rec_len, fr.len.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
-        const int grid_r = (int)std::min<uint32_t>(tiles, (uint32_t)h->sm_count * 8);
-        dm_k_logs_walk<<<n_chunks, DML_THREADS, 0, st>>>(a);
+        dm_k_logs_walk<<<a.n_chunks, DML_THREADS, 0, st>>>(a);
         dm_k_logs_scan<<<1, DML_THREADS, 0, st>>>(a);
-        dm_k_logs_compact<<<grid_r, DML_THREADS, 0, st>>>(a);
+        dm_k_logs_compact<<<dm_grid(n_records, DML_THREADS, (uint64_t)h->sm_count * 8), DML_THREADS, 0, st>>>(a);
         h->launches += 3;
         if (copy) {
-            // the copy grid covers the largest compacted size this message can have (the total is not known yet)
-            const uint64_t stores = (std::max<uint64_t>(nbytes, 1) + DML_SLACK + 15) / 16;
-            const int grid_c = (int)std::min<uint64_t>((stores + DML_THREADS - 1) / DML_THREADS, (uint64_t)h->sm_count * 16);
-            dm_k_logs_copy<<<grid_c, DML_THREADS, 0, st>>>(a);
+            dm_k_logs_copy<<<dm_logs_copy_grid(nbytes, (uint64_t)h->sm_count * 16), DML_THREADS, 0, st>>>(a);
             h->launches++;
         }
         DM_CUDA(cudaGetLastError());
@@ -916,22 +884,21 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     rc = dm_logs_unwrap(h, buf, nbytes, fr, n_train_records, true, &a, &d_rscores, &d_rflags);
     if (rc != DM_OK) return rc;
     cudaStream_t st = h->stream;
-    const uint32_t tiles = (n_records + DML_THREADS - 1) / DML_THREADS;
     DM_CUDA(cudaStreamSynchronize(st));
     const DmLogsHeader lh = *h->h_lhdr;
     if (lh.n_lines) {
         uint64_t n_lines = 0, n_anoms = 0;
         rc = dm_process_lines(h, h->d_logs_text, lh.total_bytes, 1, lh.n_train, nullptr, nullptr, 0, 0, &n_lines, &n_anoms, st);
         dm_break_chain(h, st);
-        h->last_src = DM_SRC_NONE;                            // (its anomaly list is rewritten to records below)
+        h->last_src = DMA_SRC_NONE;                           // (its anomaly list is rewritten to records below)
         if (rc != DM_OK) return rc;
         if (n_lines != lh.n_lines)
             return dm_fail(DM_ERR_STATE, "the line path found %llu records in %llu unwrapped texts", (unsigned long long)n_lines, (unsigned long long)lh.n_lines);
     } else {
         DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
-        h->last_src = DM_SRC_NONE;
+        h->last_src = DMA_SRC_NONE;
     }
-    const int grid_s = (int)std::max<uint32_t>(1, std::min<uint32_t>(std::max<uint32_t>(tiles, h->anomaly_cap / DML_THREADS), (uint32_t)h->sm_count * 8));
+    const unsigned grid_s = dm_logs_scatter_grid(n_records, h->anomaly_cap, (uint64_t)h->sm_count * 8);
     dm_k_logs_scatter<<<grid_s, DML_THREADS, 0, st>>>(a, h->d_flags, h->d_scores, d_rflags, d_rscores, h->d_anoms, h->anomaly_cap,
                                                      h->d_hdr, h->d_stats, nbytes);
     h->launches++;
@@ -943,7 +910,7 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     if (n_records_out) *n_records_out = n_records;
     if (n_malformed_out) *n_malformed_out = n_records - lh.n_lines;
     if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
-    h->last_src = DM_SRC_LOGS;                                // (the line path left last_buf / last_nbytes: the texts)
+    h->last_src = DMA_LOGS;                                   // (the line path left last_buf / last_nbytes: the texts)
     h->last_scores = d_rscores;
     return DM_OK;
 }
@@ -951,8 +918,6 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
 // ---------------------------------------------------------------------------------------
 // DetectorSchema alerts of raw-line batches, encoded on the device (dm_kernels_alerts.cuh)
 // ---------------------------------------------------------------------------------------
-static uint64_t dm_alert_tiles(uint64_t n) { return (n + DMA_TILE - 1) / DMA_TILE; }
-
 // The encoder's copy of the log_format (when both the format and the alert format are set): the matcher's own, keeping
 // the Time capture as well.
 static int dm_alert_efmt_upload(dm_handle* h) {
@@ -988,15 +953,13 @@ extern "C" int dm_set_alert_format(dm_handle* h, uint32_t n_strings, const uint8
         // everything the encoder needs, once: per record a rank, per anomaly-list entry a record's line, mask, offset and
         // size, the scan's tile sums.  Allocated into locals and kept only when every allocation succeeded, so that a
         // failed call leaves the handle without an encoder (and a later call allocates again).
-        const uint64_t lines = h->max_lines + 1, recs = (uint64_t)h->anomaly_cap + 1;
-        const uint64_t tiles = dm_alert_tiles(std::max(lines, recs)) + 1;
         DmAlertFmt* d_afmt = nullptr;
         DmAlertHeader *d_ahdr = nullptr, *h_ahdr = nullptr;
         void* d_alert = nullptr;
         e = cudaMalloc(&d_afmt, sizeof(DmAlertFmt));
         if (e == cudaSuccess) e = cudaMalloc(&d_ahdr, sizeof(DmAlertHeader));
         if (e == cudaSuccess) e = cudaHostAlloc(&h_ahdr, sizeof(DmAlertHeader), cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaMalloc(&d_alert, 4 * lines + 8 + 8 * recs * 3 + 8 * tiles);
+        if (e == cudaSuccess) e = cudaMalloc(&d_alert, dm_alert_scratch(nullptr, h->max_lines, h->anomaly_cap, nullptr, nullptr));
         if (e == cudaSuccess) {
             h->d_afmt = d_afmt; h->d_ahdr = d_ahdr; h->h_ahdr = h_ahdr; h->d_alert = d_alert;
         } else {
@@ -1030,7 +993,7 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     if (!h || !out_len || !n_alerts || !declined) return dm_fail(DM_ERR_ARG, "NULL argument");
     if (out_cap && !out) return dm_fail(DM_ERR_ARG, "out is NULL");
     if (!h->d_afmt || !h->d_aout) return dm_fail(DM_ERR_STATE, "dm_set_alert_format has not been called");
-    if (h->last_src == DM_SRC_NONE)
+    if (h->last_src == DMA_SRC_NONE)
         return dm_fail(DM_ERR_STATE, "the last batch did not come from dm_process_lines, dm_process_logs or dm_process_records");
     *out_len = 0;
     *n_alerts = 0;
@@ -1038,66 +1001,58 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     int rc = dm_sync(h, nullptr, nullptr);
     if (rc != DM_OK) return rc;
     const uint32_t src = h->last_src;
-    const bool records = src == DM_SRC_RECORDS;
-    // raw lines and LogSchema: the anomaly list (in record space after dm_k_logs_scatter); ParserSchema: the flags
-    const uint64_t n_lines = records ? h->last_n_records : h->h_hdr->n_lines;
-    const uint64_t n_flagged = records ? h->h_hdr->n_anomalies : std::min(h->h_hdr->anomaly_list_count, h->anomaly_cap);
-    if (n_flagged == 0 || n_lines == 0) return DM_OK;
-    if (n_flagged > h->anomaly_cap) {                         // more anomalous records than the per-record arrays hold
+    uint64_t n_lines;
+    bool over;
+    const uint64_t n_flagged = dm_alert_entries(src, *h->h_hdr, h->last_n_records, h->anomaly_cap, &n_lines, &over);
+    if (over) {
         *n_alerts = n_flagged;
         *declined = 1;
         return DM_OK;
     }
+    if (n_flagged == 0) return DM_OK;
     const uint32_t entries = (uint32_t)n_flagged;
     cudaStream_t st = h->last_stream;
     dm_break_chain(h, st);
-    const uint64_t lines = h->max_lines + 1, recs = (uint64_t)h->anomaly_cap + 1;
     DmAlertArgs a;
+    unsigned long long* tile_sums;
+    dm_alert_scratch((uint8_t*)h->d_alert, h->max_lines, h->anomaly_cap, &a, &tile_sums);
     a.fmt = h->d_afmt; a.buf = h->last_buf; a.nbytes = h->last_nbytes; a.scores = h->last_scores;
     a.anoms = h->d_anoms; a.n_entries = entries; a.n_lines = n_lines;
-    a.rank = (uint32_t*)h->d_alert;
-    unsigned long long* w = (unsigned long long*)((uint8_t*)h->d_alert + ((4 * lines + 7) & ~7ull));
-    a.rec_off = w; a.size = w + recs;
-    unsigned long long* tile_sums = w + 2 * recs;
-    a.rec_line = (uint32_t*)(tile_sums + dm_alert_tiles(std::max(lines, recs)) + 1);
-    a.rec_mask = a.rec_line + recs;
     a.ahdr = h->d_ahdr; a.first_log_id = first_log_id; a.first_alert_id = first_alert_id; a.now = now;
     a.out = h->d_aout; a.out_cap = std::min(out_cap, h->alert_cap);
     a.efmt = h->d_efmt; a.nbuf = h->d_norm;
-    if (src == DM_SRC_LOGS) {
+    a.src = src;
+    if (src == DMA_LOGS) {
         float* rscores;
         uint8_t* rflags;
-        const DmLogsArgs la = dm_logs_args(h, &rscores, &rflags);
-        a.src = DMA_LOGS; a.pay = h->d_in; a.pay_off = la.rec_off; a.pay_len = la.rec_len;
+        const DmLogsArgs la = dm_logs_carve(h->d_logs, h->logs_cap, h->logs_chunks, h->d_lhdr, &rscores, &rflags);
+        a.pay = h->d_in; a.pay_off = la.rec_off; a.pay_len = la.rec_len;
         a.log_line = la.rec_line; a.log_dst = la.line_dst;
-    } else if (records) {
-        a.src = DMA_RECORDS; a.pay = h->d_in; a.pay_off = h->d_vals; a.pay_len = h->d_vals + n_lines;
+    } else if (src == DMA_RECORDS) {
+        a.pay = h->d_in; a.pay_off = h->d_vals; a.pay_len = h->d_vals + n_lines;
         a.scores = h->d_scores; a.flags = h->d_flags; a.masks = h->d_masks; a.mons = h->d_mons;
     }
+    bool fmtl;
+    uint64_t mark_n;
+    const DmAlertKernel k_mark = dm_alert_mark_kernel(src, false, n_lines, entries, &mark_n);
+    const DmAlertKernel k_gather = dm_alert_mark_kernel(src, true, n_lines, entries, &mark_n);
+    const DmAlertKernel k_size = dm_alert_pass_kernel(src, h->fmt_set, h->fmt_norm, false, &fmtl);
+    const DmAlertKernel k_write = dm_alert_pass_kernel(src, h->fmt_set, h->fmt_norm, true, &fmtl);
     // log_format mode: the size and write passes re-run the matcher (one thread per record, DM_FMTL_THREADS per CTA)
-    const bool fmt = h->fmt_set && !records, norm = h->fmt_norm;
-    if (fmt && !h->d_efmt) return dm_fail(DM_ERR_STATE, "no log_format for the alert encoder");
-    const size_t fsmem = (size_t)2 * h->efmt_slots * DM_FMTL_THREADS * sizeof(uint2);
-    const int fgrid = (int)std::max<uint32_t>(1, std::min<uint32_t>((entries + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS, (uint32_t)h->sm_count * 32));
-    const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>((entries + DMA_THREADS - 1) / DMA_THREADS, (uint32_t)h->sm_count * 8));
-    const int rgrid = (int)std::max<uint64_t>(1, std::min<uint64_t>((n_lines + DMA_THREADS - 1) / DMA_THREADS, (uint64_t)h->sm_count * 8));
+    if (fmtl && !h->d_efmt) return dm_fail(DM_ERR_STATE, "no log_format for the alert encoder");
+    const unsigned mgrid = dm_grid(mark_n, DMA_THREADS, (uint64_t)h->sm_count * 8);
+    const unsigned threads = fmtl ? DM_FMTL_THREADS : DMA_THREADS;
+    const unsigned pgrid = dm_grid(entries, threads, (uint64_t)h->sm_count * (fmtl ? 32 : 8));
+    const size_t smem = fmtl ? (size_t)2 * h->efmt_slots * DM_FMTL_THREADS * sizeof(uint2) : 0;
     DM_CUDA(cudaMemsetAsync(h->d_ahdr, 0, sizeof(DmAlertHeader), st));
     DM_CUDA(cudaMemsetAsync(a.rank, 0, n_lines * 4, st));
     DM_CUDA(cudaMemsetAsync(a.rec_mask, 0, (uint64_t)entries * 4, st));
-    if (records) dm_k_alert_mark_records<<<rgrid, DMA_THREADS, 0, st>>>(a);
-    else dm_k_alert_mark<<<grid, DMA_THREADS, 0, st>>>(a);
+    k_mark<<<mgrid, DMA_THREADS, 0, st>>>(a);
     dm_alert_scan<uint32_t>(a.rank, n_lines, (uint32_t*)tile_sums, &h->d_ahdr->n_alerts, st);
-    if (records) dm_k_alert_gather_records<<<rgrid, DMA_THREADS, 0, st>>>(a);
-    else dm_k_alert_gather<<<grid, DMA_THREADS, 0, st>>>(a);
-    if (records) dm_k_alert_records<false><<<grid, DMA_THREADS, 0, st>>>(a);
-    else if (!fmt) dm_k_alert_size<<<grid, DMA_THREADS, 0, st>>>(a);
-    else if (norm) dm_k_alert_format<true, false><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
-    else dm_k_alert_format<false, false><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
+    k_gather<<<mgrid, DMA_THREADS, 0, st>>>(a);
+    k_size<<<pgrid, threads, smem, st>>>(a);
     dm_alert_scan<unsigned long long>(a.size, entries, tile_sums, &h->d_ahdr->total, st);
-    if (records) dm_k_alert_records<true><<<grid, DMA_THREADS, 0, st>>>(a);
-    else if (!fmt) dm_k_alert_write<<<grid, DMA_THREADS, 0, st>>>(a);
-    else if (norm) dm_k_alert_format<true, true><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
-    else dm_k_alert_format<false, true><<<fgrid, DM_FMTL_THREADS, fsmem, st>>>(a);
+    k_write<<<pgrid, threads, smem, st>>>(a);
     h->launches += 10;
     DM_CUDA(cudaGetLastError());
     DM_CUDA(cudaMemcpyAsync(h->h_ahdr, h->d_ahdr, sizeof(DmAlertHeader), cudaMemcpyDeviceToHost, st));
@@ -1156,34 +1111,30 @@ extern "C" int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, 
     int rc = dm_logs_frames(h, buf, nbytes, delimited, &fr);
     if (rc != DM_OK) return rc;
     const uint32_t n_records = (uint32_t)fr.off.size();
-    h->last_src = DM_SRC_NONE;                                // (d_in no longer holds the last detected batch)
+    h->last_src = DMA_SRC_NONE;                               // (d_in no longer holds the last detected batch)
     DmLogsArgs la;
     float* rscores;
     uint8_t* rflags;
     rc = dm_logs_unwrap(h, buf, nbytes, fr, 0, false, &la, &rscores, &rflags);
     if (rc != DM_OK) return rc;
     cudaStream_t st = h->stream;
-    const uint64_t tiles = dm_alert_tiles(n_records) + 1;
-    if (n_records + tiles + 1 > h->psize_cap) {
+    const uint64_t words = dm_parse_scratch(nullptr, n_records, nullptr, nullptr, nullptr);
+    if (words > h->psize_cap) {
         DM_CUDA(cudaStreamSynchronize(st));
         cudaFree(h->d_psize);
         h->d_psize = nullptr;
         h->psize_cap = 0;
-        const uint64_t cap = std::max<uint64_t>(2 * (n_records + tiles + 1), 8192);
+        const uint64_t cap = std::max<uint64_t>(2 * words, 8192);
         DM_CUDA(cudaMalloc(&h->d_psize, cap * sizeof(unsigned long long)));
         h->psize_cap = cap;
     }
-    DmParseArgs a;
-    a.pf = h->d_pf; a.pfmt = h->d_pfmt; a.buf = h->d_in; a.nbuf = h->d_norm; a.n_records = n_records;
-    a.rec_off = la.rec_off; a.rec_len = la.rec_len; a.text_off = la.text_off; a.text_len = la.text_len; a.rank = la.rec_line;
-    a.size = h->d_psize; a.first_id = first_parsed_id; a.now = now;
-    unsigned long long* tile_sums = h->d_psize + n_records;
-    unsigned long long* d_total = tile_sums + tiles;
-    a.total = d_total;
+    DmParseArgs a = dm_parse_args(la, h->d_pf, h->d_pfmt, h->d_norm, first_parsed_id, now);
+    unsigned long long *tile_sums, *d_total;
+    dm_parse_scratch(h->d_psize, n_records, &a, &tile_sums, &d_total);
     const bool norm = h->fmt_norm;
     if (norm && !h->d_norm) return dm_fail(DM_ERR_STATE, "no R-norm scratch");
     const size_t smem = (size_t)2 * h->pfmt_slots * DM_FMTL_THREADS * sizeof(uint2);
-    const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>((n_records + DM_FMTL_THREADS - 1) / DM_FMTL_THREADS, (uint32_t)h->sm_count * 32));
+    const unsigned grid = dm_grid(n_records, DM_FMTL_THREADS, (uint64_t)h->sm_count * 32);
     DM_CUDA(cudaMemsetAsync(d_total, 0, sizeof(unsigned long long), st));
     if (n_records) {
         dm_parse_kernel(norm, false)<<<grid, DM_FMTL_THREADS, smem, st>>>(a);
@@ -1264,7 +1215,7 @@ extern "C" int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t n
     DM_CUDA(cudaEventRecord(sl.ev_in, h->st_in));
     cudaStream_t st = h->stream;                       // ONE compute stream: submission order = processing order
     h->last_stream = st;
-    h->last_src = DM_SRC_NONE;
+    h->last_src = DMA_SRC_NONE;
     DM_CUDA(cudaStreamWaitEvent(st, sl.ev_in, 0));
     if (nbytes == 0) DM_CUDA(cudaMemsetAsync(sl.d_hdr, 0, sizeof(DmBatchHeader), st));
     const int launched = dmx_launch(&h->dmx, sl.d_in, nbytes, n_train_lines, h->table, sl.d_flags, sl.d_scores, h->max_lines, sl.d_anoms,
@@ -1414,7 +1365,7 @@ extern "C" int dm_import_known(dm_handle* h, const uint64_t* keys, uint64_t n) {
     DM_CUDA(cudaMemcpy(d_tmp, keys, n * sizeof(unsigned long long), cudaMemcpyHostToDevice));
     DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), h->last_stream));
     dm_break_chain(h, h->last_stream);
-    h->last_src = DM_SRC_NONE;
+    h->last_src = DMA_SRC_NONE;
     dm_k_insert_keys<<<std::max(1, (int)std::min<uint64_t>((n + 255) / 256, 1024)), 256, 0, h->last_stream>>>(h->table, d_tmp, n, &h->d_hdr->error);
     DM_CUDA(cudaGetLastError());
     int rc = dm_sync(h, nullptr, nullptr);

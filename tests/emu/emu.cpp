@@ -20,6 +20,7 @@
 #include "dm_kernels_lanes.cuh"
 #include "dm_kernels_logs.cuh"
 #include "dm_kernels_alerts.cuh"
+#include "dm_kernels_parse.cuh"
 #include "dm_format_host.h"
 #include "dm_host.h"
 
@@ -54,8 +55,9 @@ void emu_launch_grid(unsigned blocks, unsigned threads, const std::function<void
 
 void emu_launch(unsigned threads, const std::function<void()>& body) { emu_launch_grid(1, threads, body); }
 
-// The emulated dm_handle: the known set, statistics, batch header and anomaly list, K_A's scratch, and the
-// configuration the emu_set_* calls leave (as dm_set_monitors / dm_set_combos / dm_set_format / dm_set_alert_format).
+// The emulated dm_handle: the known set, statistics, batch header and anomaly list, K_A's scratch, the configuration
+// the emu_set_* calls leave (as dm_set_monitors / dm_set_combos / dm_set_format / dm_set_alert_format /
+// dm_set_parser_format), and what the last batch leaves for the encoder.
 struct EmuHandle {
     DmKeys keys;
     DmTable table;
@@ -74,7 +76,27 @@ struct EmuHandle {
     std::string fmt_err;
     DmAlertFmt afmt{};
     bool afmt_set = false;
+    DmFormat efmt{};                     // the encoder's format (dm_alert_efmt_build), once fmt and afmt are set
+    DmParseFmt pf{};                     // the parser's format and the matcher's format it runs (dm_parse_efmt_build)
+    DmFormat pfmt{};
+    bool parse_set = false;              // cleared by emu_set_format, as by dm_set_format
     struct EmuStream* xs = nullptr;      // stream variant (created on first use)
+    // the last batch, as dm_encode_alerts reads it: its source (DMA_*), the message the line path read (emu_message),
+    // its scores, the ParserSchema records; a LogSchema or ParserSchema message with hostile slack (d_in), the record
+    // frames, flags, scores and masks of dm_process_records (d_vals, d_flags, d_scores, d_masks)
+    uint32_t last_src = DMA_SRC_NONE;
+    uint8_t* msg = nullptr;
+    uint64_t msg_bytes = 0;
+    const float* last_scores = nullptr;
+    uint32_t last_n_records = 0;
+    std::vector<uint8_t> in, flags;
+    std::vector<float> scores;
+    std::vector<uint32_t> vals, masks;
+    // the unwrap of the last LogSchema message: its arrays (one block, dm_logs_carve), header and compacted texts
+    std::vector<uint8_t> logs, logs_text;
+    uint64_t logs_cap = 0;
+    uint32_t logs_chunks = 0;
+    DmLogsHeader lhdr;
 };
 
 extern "C" EmuHandle* emu_create(uint32_t n_keys, const uint8_t* blob, const uint32_t* lens, uint32_t table_log2,
@@ -108,7 +130,19 @@ extern "C" EmuHandle* emu_create(uint32_t n_keys, const uint8_t* blob, const uin
 }
 
 void emu_stream_free(struct EmuStream*);
-extern "C" void emu_destroy(EmuHandle* h) { emu_stream_free(h->xs); delete h; }
+extern "C" void emu_destroy(EmuHandle* h) {
+    emu_stream_free(h->xs);
+    free(h->msg);
+    delete h;
+}
+
+// the anomaly list's capacity (dm_handle::anomaly_cap; 65536 from emu_create)
+extern "C" void emu_set_anomaly_cap(EmuHandle* h, uint32_t cap) { h->anoms.assign(cap ? cap : 1, dm_anomaly_t{}); }
+
+// as dm_alert_efmt_upload: the encoder's copy of the log_format, once both formats are set
+static void emu_efmt_build(EmuHandle* h) {
+    if (h->fmt_set && h->afmt_set) dm_alert_efmt_build(h->fmt, h->afmt.time_cap, &h->efmt);
+}
 
 // as dm_set_monitors (which also clears the combinations)
 extern "C" void emu_set_monitors(EmuHandle* h, const DmMonitor* mons, uint32_t n_mons) {
@@ -134,15 +168,30 @@ extern "C" const char* emu_set_format(EmuHandle* h, const char* log_format, cons
                                       const char* const* templates, uint32_t norm_flags) {
     h->fmt_err.clear();
     h->fmt_set = dm_format_build(log_format, content_name, n_templates, templates, norm_flags, h->mons, &h->fmt, &h->fmt_err);
-    return h->fmt_set ? nullptr : h->fmt_err.c_str();
+    if (!h->fmt_set) return h->fmt_err.c_str();
+    h->parse_set = false;
+    emu_efmt_build(h);
+    return nullptr;
 }
 
-// The message in a 64-byte aligned buffer, followed by 64 hostile bytes (slack, repeated).
-static uint8_t* emu_message(const uint8_t* msg, uint64_t nbytes, const std::vector<uint8_t>& slack) {
+// The message in a 64-byte aligned buffer, followed by 64 hostile bytes (slack, repeated); the handle keeps it as the
+// batch the line path read (dm_handle::last_buf / last_nbytes).
+static uint8_t* emu_message(EmuHandle* h, const uint8_t* msg, uint64_t nbytes, const std::vector<uint8_t>& slack) {
+    free(h->msg);
     uint8_t* buf = (uint8_t*)aligned_alloc(64, ((nbytes + 64 + 63) / 64) * 64 + 64);
-    memcpy(buf, msg, nbytes);
+    if (nbytes) memcpy(buf, msg, nbytes);
     for (uint32_t i = 0; i < 64; ++i) buf[nbytes + i] = slack[i % slack.size()];
+    h->msg = buf;
+    h->msg_bytes = nbytes;
     return buf;
+}
+
+// What dm_process_lines leaves for dm_encode_alerts besides the message: the batch's scores (copied: the caller's
+// arrays need not outlive the call) and its source.
+static void emu_lines_kept(EmuHandle* h, const float* scores, uint64_t cap) {
+    h->scores.assign(scores, scores + std::min<uint64_t>(h->hdr.n_lines, cap));
+    h->last_scores = h->scores.data();
+    h->last_src = DMA_LINES;
 }
 static const std::vector<uint8_t> EMU_KV_SLACK = {'=', '\n'};
 
@@ -177,11 +226,13 @@ static int emu_stream_run(EmuHandle* h, bool chained, const uint8_t* msg, uint64
     const uint32_t n_rows = (uint32_t)((nbytes + DMX_ROW - 1) / DMX_ROW);
     if (n_rows == 0) {
         memset(&h->hdr, 0, sizeof(h->hdr));
+        emu_message(h, msg, 0, EMU_KV_SLACK);
+        emu_lines_kept(h, scores, 0);
         *err = g_xs.sh.error;
         g_xs.sh.error = 0;
         return 0;
     }
-    uint8_t* buf = emu_message(msg, nbytes, EMU_KV_SLACK);
+    uint8_t* buf = emu_message(h, msg, nbytes, EMU_KV_SLACK);
     for (unsigned b = 0; b < DMX_NPAR; ++b) {
         if (g_xs.row_cnt[b].size() < n_rows + 1) g_xs.row_cnt[b].assign(n_rows + 1, 0xBEEF);
         if (g_xs.alerts[b].size() < h->anoms.size()) g_xs.alerts[b].resize(h->anoms.size());
@@ -217,7 +268,7 @@ static int emu_stream_run(EmuHandle* h, bool chained, const uint8_t* msg, uint64
     if (chained) emu_launch_grid(grid, DMX_THREADS, [&] { dm_k_stream<false, true>(a); });
     else emu_launch_grid(grid, DMX_THREADS, [&] { dm_k_stream<false, false>(a); });
     g_emu_last_hint = g_xs.hint;
-    free(buf);
+    emu_lines_kept(h, scores, cap);
     *n_lines = h->hdr.n_lines;
     *n_anoms = h->hdr.n_anomalies;
     *err = h->hdr.error | g_xs.sh.error;
@@ -270,8 +321,12 @@ static void emu_per_record(EmuHandle* h, const uint8_t* buf, uint64_t nbytes, ui
 extern "C" int emu_process_lanes(EmuHandle* h, const uint8_t* msg, uint64_t nbytes, uint64_t n_train, uint8_t* flags,
                                  float* scores, uint64_t cap, uint64_t* n_lines, uint64_t* n_anoms, uint32_t* err) {
     *n_lines = 0; *n_anoms = 0; *err = 0;
-    if (nbytes == 0) { memset(&h->hdr, 0, sizeof(h->hdr)); return 0; }      // as dm_process_lines: no launch at all
-    uint8_t* buf = emu_message(msg, nbytes, EMU_KV_SLACK);
+    uint8_t* buf = emu_message(h, msg, nbytes, EMU_KV_SLACK);
+    if (nbytes == 0) {                                                        // as dm_process_lines: no launch at all
+        memset(&h->hdr, 0, sizeof(h->hdr));
+        emu_lines_kept(h, scores, 0);
+        return 0;
+    }
     const bool combo = h->mons.n_combos > 0;
     const unsigned grid = dm_detect_grid(nbytes, h->max_lines, DM_LANES_THREADS, 5);
     g_emu_dyn_smem.assign((size_t)DM_MAX_KEYS * DM_LANES_THREADS * sizeof(unsigned long long), 0);
@@ -279,7 +334,7 @@ extern "C" int emu_process_lanes(EmuHandle* h, const uint8_t* msg, uint64_t nbyt
         const DmLanesKernel k = dm_lanes_kernel(train, combo);
         emu_launch_grid(grid, DM_LANES_THREADS, [&] { k(a); });
     });
-    free(buf);
+    emu_lines_kept(h, scores, cap);
     *n_lines = h->hdr.n_lines;
     *n_anoms = h->hdr.n_anomalies;
     *err = h->hdr.error;
@@ -292,7 +347,12 @@ extern "C" int emu_process_format(EmuHandle* h, const uint8_t* msg, uint64_t nby
                                   float* scores, uint64_t cap, uint64_t* n_lines, uint64_t* n_anoms, uint32_t* err) {
     if (!h->fmt_set) return -6;
     *n_lines = 0; *n_anoms = 0; *err = 0;
-    if (nbytes == 0) { memset(&h->hdr, 0, sizeof(h->hdr)); return 0; }      // as dm_process_lines: no launch at all
+    if (nbytes == 0) {                                                        // as dm_process_lines: no launch at all
+        memset(&h->hdr, 0, sizeof(h->hdr));
+        emu_message(h, msg, 0, EMU_KV_SLACK);
+        emu_lines_kept(h, scores, 0);
+        return 0;
+    }
     const DmFormat& f = h->fmt;
     // hostile slack: the bytes of the configured literals, each followed by '\n', over and over (the kernel reads up to
     // 12 bytes past a record; none of it may count)
@@ -301,7 +361,7 @@ extern "C" int emu_process_format(EmuHandle* h, const uint8_t* msg, uint64_t nby
         for (uint32_t j = 0; j < f.lit_len[i]; ++j) slack.push_back((uint8_t)(f.pool[f.lit_off[i] + j / 4] >> (8 * (j % 4))));
         slack.push_back('\n');
     }
-    uint8_t* buf = emu_message(msg, nbytes, slack);
+    uint8_t* buf = emu_message(h, msg, nbytes, slack);
     // R-norm scratch: hostile content (the kernel may only read back what it wrote itself)
     uint8_t* nbuf = (uint8_t*)aligned_alloc(64, ((nbytes + 256 + 63) / 64) * 64);
     memset(nbuf, 0xA5, nbytes + 256);
@@ -313,7 +373,7 @@ extern "C" int emu_process_format(EmuHandle* h, const uint8_t* msg, uint64_t nby
         emu_launch_grid(grid, DM_FMTL_THREADS, [&] { k(a, &f, nbuf); });
     });
     free(nbuf);
-    free(buf);
+    emu_lines_kept(h, scores, cap);
     *n_lines = h->hdr.n_lines;
     *n_anoms = h->hdr.n_anomalies;
     *err = h->hdr.error;
@@ -332,72 +392,150 @@ extern "C" int64_t emu_frame_split(const uint8_t* buf, uint64_t nbytes, uint32_t
 }
 
 // ParserSchema records, as dm_process_records: the host framing, then the train / bound / detect launches of
-// dm_k_records with the monitors and combinations of emu_set_monitors / emu_set_combos.  -1: a framing error.
+// dm_k_records with the monitors and combinations of emu_set_monitors / emu_set_combos, on the handle's copy of the
+// message and arrays (hostile to start with), the outputs then copied to flags / scores / masks.  -1: a framing error.
 extern "C" int emu_process_records(EmuHandle* h, const uint8_t* msg, uint64_t nbytes, uint32_t n_train, uint8_t* flags,
                                    float* scores, uint32_t* masks, uint64_t cap, uint64_t* n_records, uint64_t* n_anoms) {
     const DmFrames fr = dm_frame_split(msg, nbytes);
     if (fr.error) return -1;
     const uint32_t n = (uint32_t)fr.off.size();
     if (n > cap) return -4;
+    h->last_src = DMA_SRC_NONE;
     memset(&h->hdr, 0, sizeof(h->hdr));
+    h->in.assign(nbytes + 64, 0x0A);                                // hostile slack: '\n' bytes
+    if (nbytes) memcpy(h->in.data(), msg, nbytes);
+    h->vals = fr.off;                                                // offsets, then lengths (as d_vals)
+    h->vals.insert(h->vals.end(), fr.len.begin(), fr.len.end());
+    h->flags.assign(n + 1, 7);
+    h->scores.assign(n + 1, -1.0f);
+    h->masks.assign(n + 1, 0xDEADBEEFu);
     DmRecordsArgs a;
-    a.buf = msg; a.rec_off = fr.off.data(); a.rec_len = fr.len.data(); a.n_records = n; a.n_train_records = n_train;
-    a.mons = &h->mons; a.table = h->table; a.flags = flags; a.scores = scores; a.masks = masks; a.hdr = &h->hdr; a.stats = h->stats;
+    a.buf = h->in.data(); a.rec_off = h->vals.data(); a.rec_len = h->vals.data() + n; a.n_records = n; a.n_train_records = n_train;
+    a.mons = &h->mons; a.table = h->table; a.flags = h->flags.data(); a.scores = h->scores.data(); a.masks = h->masks.data();
+    a.hdr = &h->hdr; a.stats = h->stats;
     uint32_t bound[2] = {0, 0};
     if (n) {
         if (n_train > 0) {
             emu_launch(128, [&] { dm_k_records(a, 2); });
-            emu_launch(256, [&] { dm_k_records_bound(flags, n, n_train, bound); });
+            emu_launch(256, [&] { dm_k_records_bound(h->flags.data(), n, n_train, bound); });
             emu_launch(128, [&] { dm_k_records(a, 0, bound); });
         }
         if (n_train < n) emu_launch(128, [&] { dm_k_records(a, 1, n_train > 0 ? bound : nullptr); });
     }
     dm_stats_add_records(h->stats, n, bound[1], n - (n_train > 0 ? bound[0] : 0), nbytes);
+    memcpy(flags, h->flags.data(), n);
+    memcpy(scores, h->scores.data(), (uint64_t)n * 4);
+    memcpy(masks, h->masks.data(), (uint64_t)n * 4);
     *n_records = n;
     *n_anoms = h->hdr.n_anomalies;
+    h->last_src = DMA_RECORDS;
+    h->last_n_records = n;
+    h->last_scores = h->scores.data();
     return 0;
 }
 
 // ---------------------------------------------------------------------------------------------- LogSchema unwrap
-// Frames the message as dm_process_logs does, then runs the four unwrap kernels (dm_kernels_logs.cuh) with the walk
-// grid capped at `walk_ctas` CTAs (so that a CTA walks several tiles of records) and the copy on `copy_ctas` CTAs (so
-// that its threads take the grid-stride loop).  The message is followed by hostile bytes, the output buffer is
-// pre-filled with 0xEE.  Outputs: out (the compacted texts and the slack), rec_line / line_rec / line_dst, hdr =
-// {total_bytes, n_lines, n_train, bound}.  Returns the record count, or -1 for a framing error.
+// As dm_logs_unwrap, for the records fr of the message: the handle keeps the message with hostile slack ('\n' bytes)
+// and the unwrap's arrays, carved from one block that is filled with hostile bytes before each call.  The walk runs on
+// at most walk_ctas CTAs, the compact on at most 2 and (when out is set) the copy on at most copy_ctas, so that a CTA
+// walks several tiles of records and the others take their grid-stride loops.
+static void emu_unwrap(EmuHandle* h, const uint8_t* msg, uint64_t nbytes, const DmFrames& fr, uint32_t n_train,
+                       uint32_t walk_ctas, uint32_t copy_ctas, uint8_t* out, uint64_t out_cap, DmLogsArgs* a,
+                       float** rscores, uint8_t** rflags) {
+    const uint32_t n = (uint32_t)fr.off.size();
+    h->in.assign(nbytes + 64, 0x0A);
+    if (nbytes) memcpy(h->in.data(), msg, nbytes);
+    h->logs_cap = n;
+    h->logs_chunks = walk_ctas;
+    h->logs.assign(dm_logs_scratch_bytes(h->logs_cap, h->logs_chunks), 0xEE);
+    memset(&h->lhdr, 0xEE, sizeof(h->lhdr));
+    *a = dm_logs_carve(h->logs.data(), h->logs_cap, h->logs_chunks, &h->lhdr, rscores, rflags);
+    dm_logs_call(a, h->in.data(), n, n_train, walk_ctas, out, out_cap);
+    std::copy(fr.off.begin(), fr.off.end(), (uint32_t*)a->rec_off);
+    std::copy(fr.len.begin(), fr.len.end(), (uint32_t*)a->rec_len);
+    if (n) {
+        emu_launch_grid(a->n_chunks, DML_THREADS, [&] { dm_k_logs_walk(*a); });
+        emu_launch_grid(1, DML_THREADS, [&] { dm_k_logs_scan(*a); });
+        emu_launch_grid(dm_grid(n, DML_THREADS, 2), DML_THREADS, [&] { dm_k_logs_compact(*a); });
+        if (out) emu_launch_grid(dm_logs_copy_grid(nbytes, copy_ctas), DML_THREADS, [&] { dm_k_logs_copy(*a); });
+    } else {
+        memset(&h->lhdr, 0, sizeof(h->lhdr));                         // as dm_logs_unwrap's cudaMemsetAsync of d_lhdr
+    }
+}
+
+// The unwrap kernels alone: frames the message as dm_process_logs does and unwraps it (the walk on at most `walk_ctas`
+// CTAs, the copy on at most `copy_ctas`) into out, pre-filled with 0xEE.  Outputs: out (the compacted texts and the
+// slack), rec_line / line_rec / line_dst, hdr = {total_bytes, n_lines, n_train, bound}.  Returns the record count, or -1
+// for a framing error.
 extern "C" int64_t emu_logs_unwrap(const uint8_t* msg, uint64_t nbytes, int delimited, uint32_t n_train, uint32_t walk_ctas,
                                    uint32_t copy_ctas, uint8_t* out, uint64_t out_cap, uint32_t* rec_line,
                                    uint32_t* line_rec, uint32_t* line_dst, uint64_t* hdr) {
-    DmFrames fr;
-    if (delimited) {
-        fr = dm_frame_split(msg, nbytes);
-        if (fr.error) return -1;
-    } else {
-        fr.off.push_back(0);
-        fr.len.push_back((uint32_t)nbytes);
-    }
-    const uint32_t n = (uint32_t)fr.off.size();
-    std::vector<uint8_t> buf(nbytes + 64, 0x0A);                     // hostile slack: '\n' bytes
-    memcpy(buf.data(), msg, nbytes);
-    uint32_t per_cta;
-    const uint32_t n_chunks = dm_logs_plan(n, walk_ctas, &per_cta);
-    std::vector<uint32_t> text_off(n + 1), text_len(n + 1), line_src(n + 1);
-    std::vector<unsigned long long> loc(n + 1), chunk(n_chunks + 1);
-    DmLogsHeader lh;
-    memset(&lh, 0, sizeof(lh));
-    DmLogsArgs a;
-    a.buf = buf.data(); a.rec_off = fr.off.data(); a.rec_len = fr.len.data(); a.n_records = n; a.n_train_records = n_train;
-    a.per_cta = per_cta; a.n_chunks = n_chunks; a.text_off = text_off.data(); a.text_len = text_len.data();
-    a.loc = loc.data(); a.chunk = chunk.data(); a.rec_line = rec_line; a.line_src = line_src.data(); a.line_dst = line_dst;
-    a.line_rec = line_rec; a.out = out; a.out_cap = out_cap; a.lhdr = &lh;
+    const DmFrames fr = dm_frame_records(msg, nbytes, delimited != 0);
+    if (fr.error) return -1;
+    EmuHandle* h = new EmuHandle();
     memset(out, 0xEE, out_cap);
-    if (n) {
-        emu_launch_grid(n_chunks, DML_THREADS, [&] { dm_k_logs_walk(a); });
-        emu_launch_grid(1, DML_THREADS, [&] { dm_k_logs_scan(a); });
-        emu_launch_grid(2, DML_THREADS, [&] { dm_k_logs_compact(a); });
-        emu_launch_grid(copy_ctas, DML_THREADS, [&] { dm_k_logs_copy(a); });
-    }
+    DmLogsArgs a;
+    float* rscores;
+    uint8_t* rflags;
+    emu_unwrap(h, msg, nbytes, fr, n_train, walk_ctas, copy_ctas, out, out_cap, &a, &rscores, &rflags);
+    const DmLogsHeader lh = h->lhdr;
+    std::copy(a.rec_line, a.rec_line + a.n_records, rec_line);
+    std::copy(a.line_rec, a.line_rec + lh.n_lines, line_rec);
+    if (a.n_records) std::copy(a.line_dst, a.line_dst + lh.n_lines + 1, line_dst);
     hdr[0] = lh.total_bytes; hdr[1] = lh.n_lines; hdr[2] = lh.n_train; hdr[3] = lh.bound;
-    return n;
+    emu_destroy(h);
+    return a.n_records;
+}
+
+// As dm_process_logs: the framing, the unwrap (walk and copy on at most 2 CTAs), the line path of `variant` (0 stream,
+// 1 stream with the chained re-check, 2 lanes, 3 log_format) on the compacted texts, then dm_k_logs_scatter on at most 2
+// CTAs.  flags / scores: per record (cap entries).  Returns 0, -1 for a framing error, -4 when the records exceed cap,
+// or the line path's error.
+extern "C" int emu_process_logs(EmuHandle* h, int variant, const uint8_t* msg, uint64_t nbytes, int delimited, uint32_t n_train,
+                                uint8_t* flags, float* scores, uint64_t cap, uint64_t* n_records, uint64_t* n_malformed,
+                                uint64_t* n_anoms) {
+    const DmFrames fr = dm_frame_records(msg, nbytes, delimited != 0);
+    if (fr.error) return -1;
+    const uint32_t n = (uint32_t)fr.off.size();
+    if (n > cap) return -4;
+    h->logs_text.assign(dm_logs_text_bytes(nbytes), 0xEE);
+    DmLogsArgs a;
+    float* rscores;
+    uint8_t* rflags;
+    emu_unwrap(h, msg, nbytes, fr, n_train, 2, 2, h->logs_text.data(), h->logs_text.size(), &a, &rscores, &rflags);
+    const DmLogsHeader lh = h->lhdr;
+    std::vector<uint8_t> lflags(lh.n_lines + 2, 7);
+    std::vector<float> lscores(lh.n_lines + 2, -1.0f);
+    if (lh.n_lines) {
+        uint64_t nl = 0, na = 0;
+        uint32_t err = 0;
+        uint8_t* text = h->logs_text.data();
+        int rc;
+        if (variant <= 1) rc = emu_stream_run(h, variant == 1, text, lh.total_bytes, lh.n_train, lflags.data(), lscores.data(),
+                                             lh.n_lines + 2, &nl, &na, &err);
+        else if (variant == 2) rc = emu_process_lanes(h, text, lh.total_bytes, lh.n_train, lflags.data(), lscores.data(),
+                                                      lh.n_lines + 2, &nl, &na, &err);
+        else rc = emu_process_format(h, text, lh.total_bytes, lh.n_train, lflags.data(), lscores.data(), lh.n_lines + 2,
+                                     &nl, &na, &err);
+        h->last_src = DMA_SRC_NONE;                                      // (its anomaly list is rewritten to records below)
+        if (rc != 0) return rc;
+        if (err || nl != lh.n_lines) return -5;
+    } else {
+        memset(&h->hdr, 0, sizeof(h->hdr));
+        h->last_src = DMA_SRC_NONE;
+    }
+    emu_launch_grid(dm_logs_scatter_grid(n, (uint32_t)h->anoms.size(), 2), DML_THREADS, [&] {
+        dm_k_logs_scatter(a, lflags.data(), lscores.data(), rflags, rscores, h->anoms.data(), (uint32_t)h->anoms.size(),
+                          &h->hdr, h->stats, nbytes);
+    });
+    memcpy(flags, rflags, n);
+    memcpy(scores, rscores, (uint64_t)n * 4);
+    *n_records = n;
+    *n_malformed = n - lh.n_lines;
+    *n_anoms = h->hdr.n_anomalies;
+    h->last_src = DMA_LOGS;                                              // (the line path left the message: the texts)
+    h->last_scores = rscores;
+    return 0;
 }
 
 // ---------------------------------------------------------------------------------------------- DetectorSchema alerts
@@ -408,63 +546,77 @@ extern "C" const char* emu_set_alert_format(EmuHandle* h, uint32_t n_strings, co
     const char* why = dm_alert_fmt_build(h->keys, n_strings, strings, lens, bits_off, bits, n_combos, combo_off, members,
                                          time_cap, &h->afmt);
     h->afmt_set = why == nullptr;
+    emu_efmt_build(h);
     return why;
 }
 
-// As dm_encode_alerts on the last batch: msg / scores are that batch's message and scores (the emulated detect
-// functions do not keep them); fmt: the batch was detected in log_format mode (emu_set_format's format).  The
-// grid-stride kernels run on 2 CTAs, so that batches of more than 512 (log_format: 128) anomaly entries take their
-// stride loops; every scratch array, the R-norm scratch included, starts out hostile.  Returns 0, or -6 without an alert
-// format.
-extern "C" int emu_encode_alerts(EmuHandle* h, int fmt, const uint8_t* msg, uint64_t nbytes, const float* scores,
-                                 uint64_t first_log_id, int64_t first_alert_id, int64_t now, uint8_t* out, uint64_t out_cap,
-                                 uint64_t* out_len, uint64_t* n_alerts, int* declined) {
-    if (!h->afmt_set) return -6;
+// exclusive scan of d[0, n) as dm_alert_scan launches it; the sum to *total
+template <typename T>
+static void emu_scan(T* d, uint64_t n, T* tile_sums, T* total) {
+    const uint32_t nt = (uint32_t)std::max<uint64_t>(1, dm_alert_tiles(n));
+    emu_launch_grid(nt, DMA_THREADS, [&] { dm_k_alert_scan_tiles<T>(d, n, tile_sums); });
+    emu_launch(DMA_THREADS, [&] { dm_k_alert_scan_top<T>(tile_sums, nt, total); });
+    emu_launch_grid(nt, DMA_THREADS, [&] { dm_k_alert_scan_apply<T>(d, n, tile_sums); });
+}
+
+// As dm_encode_alerts on the last batch of emu_process_stream / _chain / _lanes / _format, emu_process_logs or
+// emu_process_records.  The grid-stride kernels run on at most 2 CTAs, so that batches of more than 512 (log_format:
+// 128) anomalous records take their stride loops; the scratch block, the R-norm scratch and the output start out
+// hostile.  Returns 0, or -6 without an alert format or a batch to word.
+extern "C" int emu_encode_alerts(EmuHandle* h, uint64_t first_log_id, int64_t first_alert_id, int64_t now, uint8_t* out,
+                                 uint64_t out_cap, uint64_t* out_len, uint64_t* n_alerts, int* declined) {
+    if (!h->afmt_set || h->last_src == DMA_SRC_NONE) return -6;
     *out_len = 0; *n_alerts = 0; *declined = 0;
-    const uint32_t entries = std::min<uint32_t>(h->hdr.anomaly_list_count, (uint32_t)h->anoms.size());
-    const uint64_t n_lines = h->hdr.n_lines;
-    if (entries == 0 || n_lines == 0) return 0;
-    std::vector<uint8_t> buf(nbytes + 64, 'x');                      // hostile slack: no record may reach into it
-    memcpy(buf.data(), msg, nbytes);
-    std::vector<uint32_t> rank(n_lines + 1, 0), rec_line(entries + 1, 0xDEADBEEFu), rec_mask(entries + 1, 0);
-    std::vector<unsigned long long> rec_off(entries + 1, 0xDEADBEEFull), size(entries + 1, 0xDEADBEEFull);
-    std::vector<unsigned long long> tiles(std::max<uint64_t>(n_lines, entries) / DMA_TILE + 2, 0xDEADBEEFull);
-    std::vector<uint8_t> dout(out_cap + 1, 0xEE);
-    DmAlertHeader ah;
-    memset(&ah, 0, sizeof(ah));
+    const uint32_t src = h->last_src, anomaly_cap = (uint32_t)h->anoms.size();
+    uint64_t n_lines;
+    bool over;
+    const uint64_t n_flagged = dm_alert_entries(src, h->hdr, h->last_n_records, anomaly_cap, &n_lines, &over);
+    if (over) { *n_alerts = n_flagged; *declined = 1; return 0; }
+    if (n_flagged == 0) return 0;
+    const uint32_t entries = (uint32_t)n_flagged;
     DmAlertArgs a;
-    a.fmt = &h->afmt; a.buf = buf.data(); a.nbytes = nbytes; a.scores = scores; a.anoms = h->anoms.data();
-    a.n_entries = entries; a.n_lines = n_lines; a.rank = rank.data(); a.rec_line = rec_line.data(); a.rec_mask = rec_mask.data();
-    a.rec_off = rec_off.data(); a.size = size.data(); a.ahdr = &ah; a.first_log_id = first_log_id;
-    a.first_alert_id = first_alert_id; a.now = now; a.out = dout.data(); a.out_cap = out_cap;
-    static DmFormat efmt;
-    dm_alert_efmt_build(h->fmt, h->afmt.time_cap, &efmt);
-    std::vector<uint8_t> nbuf(nbytes + 256, 0xA5);
-    a.efmt = &efmt; a.nbuf = nbuf.data();
-    const bool norm = dm_format_norm(h->fmt);
-    auto fmt_pass = [&](bool write) {
-        g_emu_dyn_smem.assign((size_t)2 * efmt.max_slots * DM_FMTL_THREADS * sizeof(uint2), 0xEE);
-        if (norm && write) emu_launch_grid(2, DM_FMTL_THREADS, [&] { dm_k_alert_format<true, true>(a); });
-        else if (norm) emu_launch_grid(2, DM_FMTL_THREADS, [&] { dm_k_alert_format<true, false>(a); });
-        else if (write) emu_launch_grid(2, DM_FMTL_THREADS, [&] { dm_k_alert_format<false, true>(a); });
-        else emu_launch_grid(2, DM_FMTL_THREADS, [&] { dm_k_alert_format<false, false>(a); });
+    unsigned long long* tile_sums;
+    std::vector<uint8_t> scratch(dm_alert_scratch(nullptr, h->max_lines, anomaly_cap, nullptr, nullptr), 0xEE);
+    dm_alert_scratch(scratch.data(), h->max_lines, anomaly_cap, &a, &tile_sums);
+    DmAlertHeader ah;
+    memset(&ah, 0, sizeof(ah));                                          // as dm_encode_alerts' cudaMemsetAsync of d_ahdr,
+    memset(a.rank, 0, n_lines * 4);                                      //   of the ranks
+    memset(a.rec_mask, 0, (uint64_t)entries * 4);                        //   and of the merged masks
+    std::vector<uint8_t> nbuf(h->msg_bytes + 256, 0xA5), dout(out_cap + 1, 0xEE);
+    a.fmt = &h->afmt; a.buf = h->msg; a.nbytes = h->msg_bytes; a.scores = h->last_scores;
+    a.anoms = h->anoms.data(); a.n_entries = entries; a.n_lines = n_lines;
+    a.ahdr = &ah; a.first_log_id = first_log_id; a.first_alert_id = first_alert_id; a.now = now;
+    a.out = dout.data(); a.out_cap = out_cap;
+    a.efmt = &h->efmt; a.nbuf = nbuf.data();
+    a.src = src;
+    if (src == DMA_LOGS) {
+        float* rscores;
+        uint8_t* rflags;
+        const DmLogsArgs la = dm_logs_carve(h->logs.data(), h->logs_cap, h->logs_chunks, &h->lhdr, &rscores, &rflags);
+        a.pay = h->in.data(); a.pay_off = la.rec_off; a.pay_len = la.rec_len;
+        a.log_line = la.rec_line; a.log_dst = la.line_dst;
+    } else if (src == DMA_RECORDS) {
+        a.pay = h->in.data(); a.pay_off = h->vals.data(); a.pay_len = h->vals.data() + n_lines;
+        a.scores = h->scores.data(); a.flags = h->flags.data(); a.masks = h->masks.data(); a.mons = &h->mons;
+    }
+    bool fmtl;
+    uint64_t mark_n;
+    const DmAlertKernel k_mark = dm_alert_mark_kernel(src, false, n_lines, entries, &mark_n);
+    const DmAlertKernel k_gather = dm_alert_mark_kernel(src, true, n_lines, entries, &mark_n);
+    const DmAlertKernel k_size = dm_alert_pass_kernel(src, h->fmt_set, dm_format_norm(h->fmt), false, &fmtl);
+    const DmAlertKernel k_write = dm_alert_pass_kernel(src, h->fmt_set, dm_format_norm(h->fmt), true, &fmtl);
+    const unsigned threads = fmtl ? DM_FMTL_THREADS : DMA_THREADS;
+    const unsigned mgrid = dm_grid(mark_n, DMA_THREADS, 2), pgrid = dm_grid(entries, threads, 2);
+    auto pass = [&](DmAlertKernel k) {
+        g_emu_dyn_smem.assign((size_t)2 * h->efmt.max_slots * DM_FMTL_THREADS * sizeof(uint2), 0xEE);
+        emu_launch_grid(pgrid, threads, [&] { k(a); });
     };
-    auto scan = [&](auto* d, uint64_t n, auto* total) {
-        using T = std::remove_pointer_t<decltype(d)>;
-        T* ts = (T*)tiles.data();
-        const uint32_t nt = (uint32_t)std::max<uint64_t>(1, (n + DMA_TILE - 1) / DMA_TILE);
-        emu_launch_grid(nt, DMA_THREADS, [&] { dm_k_alert_scan_tiles<T>(d, n, ts); });
-        emu_launch(DMA_THREADS, [&] { dm_k_alert_scan_top<T>(ts, nt, total); });
-        emu_launch_grid(nt, DMA_THREADS, [&] { dm_k_alert_scan_apply<T>(d, n, ts); });
-    };
-    emu_launch_grid(2, DMA_THREADS, [&] { dm_k_alert_mark(a); });
-    scan(rank.data(), n_lines, &ah.n_alerts);
-    emu_launch_grid(2, DMA_THREADS, [&] { dm_k_alert_gather(a); });
-    if (fmt) fmt_pass(false);
-    else emu_launch_grid(2, DMA_THREADS, [&] { dm_k_alert_size(a); });
-    scan(size.data(), (uint64_t)entries, &ah.total);
-    if (fmt) fmt_pass(true);
-    else emu_launch_grid(2, DMA_THREADS, [&] { dm_k_alert_write(a); });
+    emu_launch_grid(mgrid, DMA_THREADS, [&] { k_mark(a); });
+    emu_scan<uint32_t>(a.rank, n_lines, (uint32_t*)tile_sums, &ah.n_alerts);
+    emu_launch_grid(mgrid, DMA_THREADS, [&] { k_gather(a); });
+    pass(k_size);
+    emu_scan<unsigned long long>(a.size, entries, tile_sums, &ah.total);
+    pass(k_write);
     *n_alerts = ah.n_alerts;
     *out_len = ah.total;
     if (ah.declined || ah.total > out_cap) { *declined = 1; return 0; }
@@ -482,6 +634,73 @@ extern "C" uint32_t emu_utf8_replace(const uint8_t* s, uint32_t n, uint8_t* out)
 // The device's Time conversion: 1 and *ts = int(float(s)), or `now` where float() must raise ValueError; 0 (declined)
 // otherwise.
 extern "C" int emu_alert_time(const uint8_t* s, uint32_t n, long long now, long long* ts) { return dma_time(s, n, now, ts) ? 1 : 0; }
+
+// The device's Time conversion of the UTF-8 of a str (a ParserSchema Time): 1 and *ts = int(float(s)), or `now` where
+// float() must raise ValueError; 0 (declined) otherwise.
+extern "C" int emu_alert_time_str(const uint8_t* s, uint32_t n, long long now, long long* ts) {
+    return dma_time(s, n, now, ts, true) ? 1 : 0;
+}
+
+// ---------------------------------------------------------------------------------------------- the MatcherParser stage
+// as dm_set_parser_format, on the format of emu_set_format (set with no monitors); nullptr or the reason it refuses
+extern "C" const char* emu_set_parser_format(EmuHandle* h, uint32_t n_strings, const uint8_t* strings, const uint32_t* lens,
+                                             const uint32_t* capture_order) {
+    if (!h->fmt_set) return "emu_set_format has not been called";
+    DmParseFmt* P = new DmParseFmt;
+    const char* why = dm_parse_fmt_build(h->fmt, n_strings, strings, lens, capture_order, P);
+    if (!why) {
+        h->pf = *P;
+        dm_parse_efmt_build(h->fmt, &h->pfmt);
+        h->parse_set = true;
+    }
+    delete P;
+    return why;
+}
+
+// As dm_parse_logs: the unwrap without the text copy (walk on at most 2 CTAs), the size pass, the scan and the write
+// pass, the parse kernels on at most 2 CTAs so that batches of more than 128 records take their stride loops; the
+// scratch, the R-norm scratch and the output start out hostile.  out: out_cap bytes.  Returns 0; -1 for a framing
+// error, -6 without a parser format since the last emu_set_format, -4 when the output exceeds out_cap (*out_len then
+// tells how large).
+extern "C" int emu_parse_logs(EmuHandle* h, const uint8_t* msg, uint64_t nbytes, int delimited, int64_t first_id, int64_t now,
+                              uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_records, uint64_t* n_emitted) {
+    if (!h->parse_set) return -6;
+    const DmFrames fr = dm_frame_records(msg, nbytes, delimited != 0);
+    if (fr.error) return -1;
+    const uint32_t n = (uint32_t)fr.off.size();
+    h->last_src = DMA_SRC_NONE;                                          // (the handle's input is no detected batch)
+    DmLogsArgs la;
+    float* rscores;
+    uint8_t* rflags;
+    emu_unwrap(h, msg, nbytes, fr, 0, 2, 0, nullptr, 0, &la, &rscores, &rflags);
+    std::vector<uint8_t> nbuf(nbytes + 256, 0xA5), dout(out_cap + 1, 0xEE);
+    DmParseArgs a = dm_parse_args(la, &h->pf, &h->pfmt, nbuf.data(), first_id, now);
+    unsigned long long *tile_sums, *total;
+    std::vector<unsigned long long> scratch(dm_parse_scratch(nullptr, n, nullptr, nullptr, nullptr), 0xDEADBEEFull);
+    dm_parse_scratch(scratch.data(), n, &a, &tile_sums, &total);
+    *total = 0;                                                          // as dm_parse_logs' cudaMemsetAsync of the total
+    const bool norm = dm_format_norm(h->fmt);
+    const unsigned grid = dm_grid(n, DM_FMTL_THREADS, 2);
+    auto pass = [&](bool write) {
+        g_emu_dyn_smem.assign((size_t)2 * h->pfmt.max_slots * DM_FMTL_THREADS * sizeof(uint2), 0xEE);
+        const DmParseKernel k = dm_parse_kernel(norm, write);
+        emu_launch_grid(grid, DM_FMTL_THREADS, [&] { k(a); });
+    };
+    if (n) {
+        pass(false);
+        emu_scan<unsigned long long>(a.size, n, tile_sums, total);
+    }
+    *out_len = *total;
+    *n_records = n;
+    *n_emitted = h->lhdr.n_lines;
+    if (*total > out_cap) return -4;
+    if (*total) {
+        a.out = dout.data(); a.out_cap = out_cap;
+        pass(true);
+    }
+    memcpy(out, dout.data(), *total);
+    return 0;
+}
 
 // ---------------------------------------------------------------------------------------------- read-back
 // as dm_get_anomalies: the batch's entries merged per record, at most cap of them; their count

@@ -53,14 +53,21 @@ _SIGNATURES = {                                                   # name: (resty
     "emu_frame_split": (C.c_int64, [C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, _P64]),
     "emu_process_records": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_uint64, _P64, _P64]),
+    "emu_set_anomaly_cap": (None, [C.c_void_p, C.c_uint32]),
     "emu_logs_unwrap": (C.c_int64, [C.c_char_p, C.c_uint64, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
                                     C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "emu_process_logs": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_uint64, C.c_int, C.c_uint32, C.c_void_p,
+                                   C.c_void_p, C.c_uint64, _P64, _P64, _P64]),
     "emu_set_alert_format": (C.c_char_p, [C.c_void_p, C.c_uint32, C.c_char_p, _P32, _P32, _P32, C.c_uint32, _P32, _P32,
                                           C.c_uint32]),
-    "emu_encode_alerts": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_int64,
-                                    C.c_int64, C.c_void_p, C.c_uint64, _P64, _P64, C.POINTER(C.c_int)]),
+    "emu_encode_alerts": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int64, C.c_int64, C.c_void_p, C.c_uint64, _P64, _P64,
+                                    C.POINTER(C.c_int)]),
     "emu_utf8_replace": (C.c_uint32, [C.c_char_p, C.c_uint32, C.c_void_p]),
     "emu_alert_time": (C.c_int, [C.c_char_p, C.c_uint32, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "emu_alert_time_str": (C.c_int, [C.c_char_p, C.c_uint32, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "emu_set_parser_format": (C.c_char_p, [C.c_void_p, C.c_uint32, C.c_char_p, _P32, _P32]),
+    "emu_parse_logs": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_uint64,
+                                 _P64, _P64, _P64]),
     "emu_get_anomalies": (C.c_uint32, [C.c_void_p, C.POINTER(Anomaly), C.c_uint32]),
     "emu_get_stats": (None, [C.c_void_p, _P64]),
     "emu_export_known": (C.c_uint64, [C.c_void_p, _P64, C.c_uint64]),

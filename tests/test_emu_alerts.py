@@ -43,11 +43,10 @@ class EmuDevice:
         self.h = None
 
     def process_lines(self, buf, n_train_lines=0, copy=True):
-        self._msg = bytes(buf)
-        cap = self._msg.count(b"\n") + 2
+        buf = bytes(buf)
+        cap = buf.count(b"\n") + 2
         flags, scores = np.zeros(cap, np.uint8), np.zeros(cap, np.float32)
-        f, s = self.det.process_lines(self._msg, n_train_lines, out=(flags, scores))
-        self._scores = scores
+        f, s = self.det.process_lines(buf, n_train_lines, out=(flags, scores))
         self.last_n_anomalies = self.det.last_n_anomalies
         return f, s
 
@@ -74,9 +73,8 @@ class EmuDevice:
     def encode_alerts(self, first_log_id, first_alert_id, now):
         out = np.zeros(self.capacity + 1, np.uint8)
         ln, n, dec = C.c_uint64(), C.c_uint64(), C.c_int()
-        assert self.lib.emu_encode_alerts(self.h, int(self.variant == "format"), self._msg, len(self._msg), self._scores.ctypes.data, first_log_id,
-                                          first_alert_id, now, out.ctypes.data, self.capacity, C.byref(ln), C.byref(n),
-                                          C.byref(dec)) == 0
+        assert self.lib.emu_encode_alerts(self.h, first_log_id, first_alert_id, now, out.ctypes.data, self.capacity,
+                                          C.byref(ln), C.byref(n), C.byref(dec)) == 0
         if dec.value:
             self.declined += 1
             return None

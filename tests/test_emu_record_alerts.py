@@ -1,14 +1,10 @@
 """DetectorSchema alerts of LogSchema and ParserSchema batches encoded on the device (DESIGN.md R-alert, R-log and the
 record contract), CPU tier: the whole dm_process_logs sequence (unwrap, line path, scatter) or dm_process_records, then
 the encoder kernels of dm_kernels_alerts.cuh, run on the CPU emulator behind a stand-in for DeviceDetector.  Every
-reply must come out byte for byte as the component's host encoder writes it for the same emulated detection.
-
-The emulator entry points of these inputs live in tests/emu/emu_batch_alerts.cpp, which is emu.cpp plus them; it is
-built here into a library of its own, with emu_harness's recipe and every emu_* signature emu_harness declares."""
+reply must come out byte for byte as the component's host encoder writes it for the same emulated detection."""
 import ctypes as C
 import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
@@ -20,52 +16,12 @@ from pbgen import Gen as RecGen, frame, ld, tag, varint
 from test_emu_alerts import AUDIT, NOW, EmuDevice
 
 VARIANTS = {"stream": 0, "chain": 1, "lanes": 2, "format": 3}
-_P64 = C.POINTER(C.c_uint64)
-_SIGNATURES = {
-    "emu_batch_destroy": (None, [C.c_void_p]),
-    "emu_set_anomaly_cap": (None, [C.c_void_p, C.c_uint32]),
-    "emu_process_logs": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_uint64, C.c_int, C.c_uint32, C.c_void_p, C.c_void_p,
-                                   C.c_uint64, _P64, _P64, _P64]),
-    "emu_encode_log_alerts": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_uint64, _P64, _P64,
-                                        C.POINTER(C.c_int)]),
-    "emu_encode_record_alerts": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
-                                           C.c_int64, C.c_void_p, C.c_uint64, _P64, _P64, C.POINTER(C.c_int)]),
-    "emu_alert_time_str": (C.c_int, [C.c_char_p, C.c_uint32, C.c_longlong, C.POINTER(C.c_longlong)]),
-}
-
-
-def _build():
-    """tests/emu/_build/libemu_batch.so from emu_batch_alerts.cpp, rebuilt when a source is newer."""
-    import emu_harness
-    src = os.path.join(emu_harness.EMU, "emu_batch_alerts.cpp")
-    so = os.path.join(emu_harness.EMU, "_build", "libemu_batch.so")
-    deps = [src, os.path.join(emu_harness.EMU, "emu.cpp"), os.path.join(emu_harness.EMU, "cuda_emu.h")] + [
-        os.path.join(emu_harness.CSRC, f) for f in os.listdir(emu_harness.CSRC)]
-    if not (os.path.exists(so) and all(os.path.getmtime(d) <= os.path.getmtime(so) for d in deps)):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-DDM_EMU", "-I" + emu_harness.EMU, "-I" + emu_harness.CSRC,
-                               "-shared", "-fPIC", "-pthread", "-o", so, src])
-    return so
 
 
 @pytest.fixture(scope="module")
 def lib():
     import emu_harness
-    L = C.CDLL(_build())
-    for name, (res, args) in list(emu_harness._SIGNATURES.items()) + list(_SIGNATURES.items()):
-        fn = getattr(L, name)
-        fn.restype, fn.argtypes = res, args
-    return L
-
-
-def _emu_detector(lib, keys, variant):
-    """An emu_harness.EmuDetector whose handle lives in this module's library (its methods call self.lib)."""
-    import emu_harness
-    d = emu_harness.EmuDetector.__new__(emu_harness.EmuDetector)
-    d.lib, d.variant, d.keys, d.max_lines = lib, variant, [bytes(k) for k in keys], 1 << 20
-    lens = (C.c_uint32 * max(1, len(d.keys)))(*[len(k) for k in d.keys])
-    d.h = lib.emu_create(len(d.keys), b"".join(d.keys), lens, 14, (4 << 20) // emu_harness.TILE_BYTES + 2, d.max_lines)
-    return d
+    return emu_harness.lib()
 
 
 class EmuBatchDevice(EmuDevice):
@@ -73,10 +29,11 @@ class EmuBatchDevice(EmuDevice):
     emulator (tests only).  The handle has the component's monitors, combinations and log_format, as the real one."""
 
     def __init__(self, lib, comp, variant, capacity, anomaly_cap=None):
+        import emu_harness
         from test_format_combos import _monitor_array
         self.lib, self.capacity = lib, capacity
         self.variant = "format" if comp.logformat is not None else variant
-        self.det = _emu_detector(lib, [m.key for m in comp.monitors], self.variant)
+        self.det = emu_harness.EmuDetector([bytes(m.key) for m in comp.monitors], table_log2=14, variant=self.variant)
         self.h = self.det.h
         self.det.set_monitors(_monitor_array(comp.monitors), len(comp.monitors))
         if comp.logformat is not None:
@@ -88,11 +45,6 @@ class EmuBatchDevice(EmuDevice):
             lib.emu_set_anomaly_cap(self.h, anomaly_cap)
         self.last_n_anomalies = 0
         self.encoded = self.declined = 0
-        self._last = None
-
-    def close(self):
-        self.lib.emu_batch_destroy(self.h)                          # (also drops the handle's last LogSchema batch)
-        self.det.h = self.h = None
 
     def process_logs(self, buf, n_train_records=0, delimited=True):
         buf = bytes(buf)
@@ -105,7 +57,6 @@ class EmuBatchDevice(EmuDevice):
             raise wire.WireError("framing")
         assert rc == 0, rc
         self.last_n_anomalies = an.value
-        self._last = ("logs",)
         return flags[:n.value], scores[:n.value], bad.value
 
     def process_records(self, buf, n_train_records=0):
@@ -115,29 +66,10 @@ class EmuBatchDevice(EmuDevice):
         rc, n, an = self.det.process_records(buf, n_train_records, flags, scores, masks, cap)
         assert rc == 0, rc
         self.last_n_anomalies = an
-        self._last = ("records", buf, flags, scores, masks)
         return flags[:n], scores[:n], masks[:n]
 
     def stats(self):
         return self.det.stats()
-
-    def encode_alerts(self, first_log_id, first_alert_id, now):
-        out = np.zeros(self.capacity + 1, np.uint8)
-        ln, n, dec = C.c_uint64(), C.c_uint64(), C.c_int()
-        if self._last[0] == "logs":
-            rc = self.lib.emu_encode_log_alerts(self.h, int(self.variant == "format"), first_alert_id, now, out.ctypes.data,
-                                                self.capacity, C.byref(ln), C.byref(n), C.byref(dec))
-        else:
-            _, buf, flags, scores, masks = self._last
-            rc = self.lib.emu_encode_record_alerts(self.h, buf, len(buf), flags.ctypes.data, scores.ctypes.data,
-                                                   masks.ctypes.data, first_alert_id, now, out.ctypes.data, self.capacity,
-                                                   C.byref(ln), C.byref(n), C.byref(dec))
-        assert rc == 0, rc
-        if dec.value:
-            self.declined += 1
-            return None
-        self.encoded += 1
-        return out[:ln.value].tobytes(), n.value
 
 
 class HostOnly:

@@ -3,13 +3,11 @@
 - The host path, which is the specification, against an independent oracle: every ParserSchema decoded with
   protobuf's runtime and compared field by field with what oracle.rfmt (Python's `re`) and protobuf's LogSchema give.
 - The configuration: the reference's parser_config.yaml loads, and every refusal raises.
-- The kernels of dm_kernels_parse.cuh on the CPU emulator (tests/emu/emu_parse.cpp) behind a stand-in for
-  DeviceDetector: the component's device path must return the host path's bytes.
+- The kernels of dm_kernels_parse.cuh on the CPU emulator (tests/emu) behind a stand-in for DeviceDetector: the component's device path must return the host path's bytes.
 """
 import ctypes as C
 import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
@@ -240,35 +238,10 @@ def test_config_refusals(tmp_path, change, match):
 
 
 # ------------------------------------------------------------------------------------------ the kernels on the emulator
-_P64 = C.POINTER(C.c_uint64)
-
-
-def _build():
-    """tests/emu/_build/libemu_parse.so from emu_parse.cpp, rebuilt when a source is newer."""
-    import emu_harness
-    src = os.path.join(emu_harness.EMU, "emu_parse.cpp")
-    so = os.path.join(emu_harness.EMU, "_build", "libemu_parse.so")
-    deps = [src, os.path.join(emu_harness.EMU, "emu.cpp"), os.path.join(emu_harness.EMU, "cuda_emu.h")] + [
-        os.path.join(emu_harness.CSRC, f) for f in os.listdir(emu_harness.CSRC)]
-    if not (os.path.exists(so) and all(os.path.getmtime(d) <= os.path.getmtime(so) for d in deps)):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-DDM_EMU", "-I" + emu_harness.EMU, "-I" + emu_harness.CSRC,
-                               "-shared", "-fPIC", "-pthread", "-o", so, src])
-    return so
-
-
 @pytest.fixture(scope="module")
 def emu():
     import emu_harness
-    L = C.CDLL(_build())
-    for name, (res, args) in emu_harness._SIGNATURES.items():
-        fn = getattr(L, name)
-        fn.restype, fn.argtypes = res, args
-    L.emu_parse_logs.restype = C.c_int
-    L.emu_parse_logs.argtypes = [C.c_void_p, C.c_uint32, C.c_char_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
-                                 C.c_char_p, C.c_uint64, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_uint64, _P64, _P64,
-                                 _P64, C.POINTER(C.c_char_p)]
-    return L
+    return emu_harness.lib()
 
 
 class EmuParseDevice:
@@ -276,36 +249,36 @@ class EmuParseDevice:
     set up as the component sets up its own (no monitors, its log_format, its parser format)."""
 
     def __init__(self, L, comp):
+        import emu_harness
         lf = comp.logformat
         self.L = L
-        self.h = L.emu_create(0, b"", (C.c_uint32 * 1)(0), 10, 4, 1 << 20)
-        L.emu_set_monitors(self.h, None, 0)
+        self.det = emu_harness.EmuDetector([], table_log2=10)
+        self.h = self.det.h
+        self.det.set_monitors(None, 0)
         ts = list(lf.template_sources)
-        err = L.emu_set_format(self.h, lf.source.encode(), lf.content_name.encode(), len(ts),
-                               (C.c_char_p * max(1, len(ts)))(*ts), lf.flags)
-        assert not err, err
+        self.det.set_format(lf.source, ts, lf.flags, lf.content_name.encode())
         strs, order = parser_format_strings("1.0.0", comp.method_type, comp.parser_id, ts, lf.header.names)
-        self.strs = (b"".join(strs), (C.c_uint32 * len(strs))(*[len(s) for s in strs]), len(strs),
-                     (C.c_uint32 * max(1, len(order)))(*order))
+        why = L.emu_set_parser_format(self.h, len(strs), b"".join(strs), (C.c_uint32 * len(strs))(*[len(s) for s in strs]),
+                                      (C.c_uint32 * max(1, len(order)))(*order))
+        assert why is None, why
 
     def close(self):
-        self.L.emu_destroy(self.h)
+        self.det.close()
 
     def parse_logs(self, buf, delimited, first_parsed_id, now):
         buf = bytes(buf)
-        blob, lens, n_str, order = self.strs
         cap = 4 * len(buf) + 4096
         while True:
             out = np.zeros(cap, np.uint8)
-            out_len, n_rec, n_emit, why = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_char_p()
-            rc = self.L.emu_parse_logs(self.h, n_str, blob, lens, order, buf, len(buf), int(delimited), first_parsed_id, now,
-                                       out.ctypes.data, cap, C.byref(out_len), C.byref(n_rec), C.byref(n_emit), C.byref(why))
+            out_len, n_rec, n_emit = C.c_uint64(), C.c_uint64(), C.c_uint64()
+            rc = self.L.emu_parse_logs(self.h, buf, len(buf), int(delimited), first_parsed_id, now, out.ctypes.data, cap,
+                                       C.byref(out_len), C.byref(n_rec), C.byref(n_emit))
             if rc != -4:
                 break
             cap = out_len.value
         if rc == -1:
             raise wire.WireError("framing")
-        assert rc == 0, (rc, why.value)
+        assert rc == 0, rc
         return out[:out_len.value].tobytes(), n_rec.value, n_emit.value, n_rec.value - n_emit.value
 
 
