@@ -34,9 +34,9 @@ parser_schema | parser_schema_batch), or named (log_schema | log_schema_batch, n
                 Replies as for ParserSchema input; alerts carry the record's logID.
 
 Alerts of raw-line, LogSchema and ParserSchema batches with at least DEVICE_ALERTS_MIN anomalous records are encoded
-on the device (dm_encode_alerts, rule R-alert in DESIGN.md), byte for byte what the host encoder here writes; the host
-encoder words the rest, every batch the device declines, the two-slot pipelined path and single ParserSchema records
-of B200NewValueDetector.
+on the device (dm_encode_alerts, rule R-alert in DESIGN.md), byte for byte what the host encoder here writes; on the
+two-slot pipelined path of large raw-line messages each piece is such a batch.  The host encoder words the rest, every
+batch the device declines and single ParserSchema records of B200NewValueDetector.
 
 All detection decisions are taken on the device; there is no CPU path (DeviceDetector
 raises without a GPU).
@@ -465,10 +465,16 @@ class B200NewValueDetector(CoreComponent):
     # measured, so the three inputs share this threshold.
     DEVICE_ALERTS_MIN = 8
 
-    def _detect_pipelined(self, data):
-        """Detection-only message, key=value records: cut it at record boundaries into ~4 MiB pieces and run them
-        through the library's two-slot path (dm_submit_lines / dm_collect): piece k+1 crosses PCIe while piece k is
-        in the kernel.  Returns (flags, scores, anomalies or None) exactly as one dm_process_lines call would."""
+    def _detect_pipelined(self, data, base: int):
+        """Detection-only message, key=value records: cut it at record boundaries into PIPE_PIECE_BYTES pieces and run
+        them through the library's two-slot path (dm_submit_lines / dm_collect): piece k+1 crosses PCIe while piece k is
+        in the kernel.  Returns (flags, scores, pieces): flags and scores exactly as one dm_process_lines call would give
+        them; pieces (None for compact output) has one entry per piece with anomalous records, in order.  A piece with at
+        least DEVICE_ALERTS_MIN of them is encoded on the device between its collect and the next submit on its slot,
+        which rewrites the slot: its entry is (varint-delimited DetectorSchemas, count).  Any other piece, or one the
+        device declines, is left to the host encoder: its entry is the list of its anomalies as (record index in the
+        message, mask, byte offset in the message).  base: the message's first record number; the device pieces are
+        numbered as if every earlier piece's alerts were already counted in n_alerts, which the caller then does."""
         arr = np.frombuffer(data, dtype=np.uint8)
         n = int(arr.size)
         cuts = [0]
@@ -483,30 +489,49 @@ class B200NewValueDetector(CoreComponent):
         cuts.append(n)
         k = len(cuts) - 1
         det = self.det
-        want_anoms = self.output_format != "compact"
-        parts_f, parts_s, anoms, line_base = [], [], [], [0]
+        want_alerts = self.output_format != "compact"
+        parts_f, parts_s, pieces = [], [], []
+        line_base, numbered = [0], [0]                     # records and alerts of the pieces collected so far
 
         def collect(i):
             f, s = det.collect(i & 1)
-            if want_anoms and det.last_n_anomalies:
-                anoms.extend((ln + line_base[0], mask, off + cuts[i]) for ln, mask, off in det.collect_anomalies(i & 1))
+            n_anom = det.last_n_anomalies
+            if want_alerts and n_anom:
+                enc = None
+                if n_anom >= self.DEVICE_ALERTS_MIN:
+                    enc = self._device_alerts(base + line_base[0], int(f.size),
+                                              first_alert_id=self.start_id + self.n_alerts + numbered[0])
+                if enc is None:
+                    enc = [(ln + line_base[0], mask, off + cuts[i]) for ln, mask, off in det.collect_anomalies(i & 1)]
+                    numbered[0] += len(enc)
+                else:
+                    numbered[0] += enc[1]
+                pieces.append(enc)
             parts_f.append(f.copy())
             parts_s.append(s.copy())
             line_base[0] += int(f.size)
-        for i in range(k):
-            if i >= 2:
-                collect(i - 2)
-            det.submit(arr[cuts[i]:cuts[i + 1]], 0, i & 1)
-        for i in range(max(0, k - 2), k):
-            collect(i)
-        return np.concatenate(parts_f), np.concatenate(parts_s), (anoms if want_anoms else None)
+        try:
+            for i in range(k):
+                if i >= 2:
+                    collect(i - 2)
+                det.submit(arr[cuts[i]:cuts[i + 1]], 0, i & 1)
+            for i in range(max(0, k - 2), k):
+                collect(i)
+        except BaseException:
+            for slot in (0, 1):                            # leave no slot in flight for the next message
+                try:
+                    det.collect(slot)
+                except Exception:
+                    pass
+            raise
+        return np.concatenate(parts_f), np.concatenate(parts_s), (pieces if want_alerts else None)
 
     def _process_lines_one(self, data: bytes, force_delimited: bool = False) -> Optional[bytes]:
         remaining = max(0, self.data_use_training - self.n_seen)
-        anomalies = None
+        pieces = None
         if (remaining == 0 and len(data) >= self.PIPE_MIN_BYTES and self.logformat is None and not getattr(self, "combos", None)
                 and os.environ.get("DM_KERNEL", "stream") == "stream"):
-            flags, scores, anomalies = self._detect_pipelined(data)
+            flags, scores, pieces = self._detect_pipelined(data, self.n_seen)
             n_anom = int(np.count_nonzero(flags))
         else:
             try:
@@ -522,12 +547,31 @@ class B200NewValueDetector(CoreComponent):
             return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
         if n_anom == 0:
             return None
-        if anomalies is None and n_anom >= self.DEVICE_ALERTS_MIN:
-            enc = self._device_alerts(base, n)
-            if enc is not None:
-                return self._device_reply(enc, bare=n == 1 and not force_delimited)
-        if anomalies is None:
-            anomalies = self.det.anomalies()
+        bare = n == 1 and not force_delimited
+        if pieces is None:
+            if n_anom >= self.DEVICE_ALERTS_MIN:
+                enc = self._device_alerts(base, n)
+                if enc is not None:
+                    return self._device_reply(enc, bare=bare)
+            return self._host_line_reply(data, self.det.anomalies(), base, scores, bare)
+        # a pipelined message: the pieces' varint-delimited alerts in order, the host wording those the device did not
+        blobs = []
+        for p in pieces:
+            if isinstance(p, tuple):
+                blobs.append(p[0])
+                self.n_alerts += p[1]
+            else:
+                blobs.append(self._host_line_reply(data, p, base, scores, False) or b"")
+        blob = b"".join(blobs)
+        if not blob:
+            return None
+        if bare:
+            _ln, pos = wire._read_varint(blob, 0)
+            return blob[pos:]
+        return blob
+
+    def _host_line_reply(self, data, anomalies, base: int, scores, bare: bool) -> Optional[bytes]:
+        """The host encoder's reply for raw-line anomalies (record index, mask, byte offset in data)."""
         out = []
         raw_keys = [m.key for m in self.monitors]
         for line_idx, mask, offset in anomalies:
@@ -542,7 +586,7 @@ class B200NewValueDetector(CoreComponent):
                                              _alerts.record_time(rec)))
         if not out:
             return None
-        return out[0] if (n == 1 and not force_delimited) else wire.frame_delimited(out)
+        return out[0] if bare else wire.frame_delimited(out)
 
     def _count_dropped_training(self, err: Exception, remaining: int, count) -> None:
         """A training message the device refused because the known-set table is full (DM_ERR_TABLE_FULL) is dropped by
@@ -582,16 +626,19 @@ class B200NewValueDetector(CoreComponent):
             by_key.setdefault(m.alert_key, []).append(i)
         return sorted(by_key.items())
 
-    def _device_alerts(self, first_log_id: int, n_records: int) -> Optional[Tuple[bytes, int]]:
-        """The alerts of the last batch -- raw lines, LogSchema or ParserSchema records -- encoded on the device (DESIGN.md
-        R-alert): (varint-delimited DetectorSchemas, count), or None when the host encodes them -- the device declined
-        the batch, the handle has no encoder (a stand-in), or an ID does not fit the device's 64-bit integers.
-        first_log_id numbers raw lines; the other two carry their records' logIDs and pass 0."""
+    def _device_alerts(self, first_log_id: int, n_records: int,
+                       first_alert_id: Optional[int] = None) -> Optional[Tuple[bytes, int]]:
+        """The alerts of the last batch -- raw lines (a collected pipeline slot too), LogSchema or ParserSchema records --
+        encoded on the device (DESIGN.md R-alert): (varint-delimited DetectorSchemas, count), or None when the host
+        encodes them -- the device declined the batch, the handle has no encoder (a stand-in), or an ID does not fit the
+        device's 64-bit integers.  first_log_id numbers raw lines; the other two carry their records' logIDs and pass 0.
+        first_alert_id: the first alert's number (default start_id + n_alerts)."""
         det = self.det
         if not hasattr(det, "encode_alerts"):
             return None
         now = int(self.clock())
-        first_alert_id = self.start_id + self.n_alerts
+        if first_alert_id is None:
+            first_alert_id = self.start_id + self.n_alerts
         if not (-(1 << 63) <= now < (1 << 63) and -(1 << 63) <= first_alert_id and first_alert_id + n_records < (1 << 63)
                 and 0 <= first_log_id and first_log_id + n_records < (1 << 64)):
             return None

@@ -155,6 +155,10 @@ struct dm_handle {
     std::vector<cudaEvent_t> ev;         // pairs: ev[2i] start, ev[2i+1] stop
     size_t ev_used = 0;
     uint64_t launches = 0;               // kernels launched since dm_create
+    // A last batch that dm_collect made (dm_encode_alerts): the slot's, for as long as last_src is DMA_LINES and
+    // last_buf is that slot's input; every other call that makes or clears a last batch changes one of the two.
+    int last_slot = -1;
+    uint64_t slot_nbytes[2] = {0, 0};    // the message each slot was submitted last
 };
 
 static const size_t DM_PROFILE_PAIRS = 4096;
@@ -994,16 +998,27 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     if (out_cap && !out) return dm_fail(DM_ERR_ARG, "out is NULL");
     if (!h->d_afmt || !h->d_aout) return dm_fail(DM_ERR_STATE, "dm_set_alert_format has not been called");
     if (h->last_src == DMA_SRC_NONE)
-        return dm_fail(DM_ERR_STATE, "the last batch did not come from dm_process_lines, dm_process_logs or dm_process_records");
+        return dm_fail(DM_ERR_STATE, "the last batch did not come from dm_process_lines, dm_process_logs, dm_process_records "
+                                     "or dm_collect");
     *out_len = 0;
     *n_alerts = 0;
     *declined = 0;
-    int rc = dm_sync(h, nullptr, nullptr);
-    if (rc != DM_OK) return rc;
+    // A collected slot: its kernels have finished (dm_collect waited for them) and its header is the one dm_collect
+    // read; dm_sync would put the handle's own header in its place.  The encoder runs on the slot's output stream, so
+    // the other slot's kernels, in flight on the compute stream, keep running and their overlap chain stays intact.
+    const bool from_slot = h->last_src == DMA_LINES && h->last_slot >= 0 && h->last_buf == h->slots[h->last_slot].d_in;
+    const dm_handle::Slot* sl = from_slot ? &h->slots[h->last_slot] : nullptr;
+    if (sl) {
+        DM_CUDA(cudaSetDevice(h->device));
+    } else {
+        const int rc = dm_sync(h, nullptr, nullptr);
+        if (rc != DM_OK) return rc;
+    }
     const uint32_t src = h->last_src;
     uint64_t n_lines;
     bool over;
-    const uint64_t n_flagged = dm_alert_entries(src, *h->h_hdr, h->last_n_records, h->anomaly_cap, &n_lines, &over);
+    const uint64_t n_flagged = dm_alert_entries(src, sl ? *sl->h_hdr : *h->h_hdr, h->last_n_records, h->anomaly_cap, &n_lines,
+                                                &over);
     if (over) {
         *n_alerts = n_flagged;
         *declined = 1;
@@ -1011,13 +1026,13 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     }
     if (n_flagged == 0) return DM_OK;
     const uint32_t entries = (uint32_t)n_flagged;
-    cudaStream_t st = h->last_stream;
+    cudaStream_t st = sl ? sl->st_out : h->last_stream;
     dm_break_chain(h, st);
     DmAlertArgs a;
     unsigned long long* tile_sums;
     dm_alert_scratch((uint8_t*)h->d_alert, h->max_lines, h->anomaly_cap, &a, &tile_sums);
     a.fmt = h->d_afmt; a.buf = h->last_buf; a.nbytes = h->last_nbytes; a.scores = h->last_scores;
-    a.anoms = h->d_anoms; a.n_entries = entries; a.n_lines = n_lines;
+    a.anoms = sl ? sl->d_anoms : h->d_anoms; a.n_entries = entries; a.n_lines = n_lines;
     a.ahdr = h->d_ahdr; a.first_log_id = first_log_id; a.first_alert_id = first_alert_id; a.now = now;
     a.out = h->d_aout; a.out_cap = std::min(out_cap, h->alert_cap);
     a.efmt = h->d_efmt; a.nbuf = h->d_norm;
@@ -1212,6 +1227,7 @@ extern "C" int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t n
     if (sl.busy) return dm_fail(DM_ERR_STATE, "slot %u was submitted and not collected yet", slot);
     if (nbytes) DM_CUDA(cudaMemcpyAsync(sl.d_in, host_buf, nbytes, cudaMemcpyHostToDevice, h->st_in));
     DM_CUDA(cudaMemsetAsync(sl.d_in + nbytes, 0, 64, h->st_in));
+    h->slot_nbytes[slot] = nbytes;
     DM_CUDA(cudaEventRecord(sl.ev_in, h->st_in));
     cudaStream_t st = h->stream;                       // ONE compute stream: submission order = processing order
     h->last_stream = st;
@@ -1251,6 +1267,12 @@ extern "C" int dm_collect(dm_handle* h, uint32_t slot, const uint8_t** flags_out
     if (scores_out) *scores_out = sl.h_scores;
     if (n_lines_out) *n_lines_out = n;
     if (n_anomalies_out) *n_anomalies_out = sl.h_hdr->n_anomalies;
+    // the slot's batch is now the last batch, for dm_encode_alerts
+    h->last_buf = sl.d_in;
+    h->last_nbytes = h->slot_nbytes[slot];
+    h->last_scores = sl.d_scores;
+    h->last_src = DMA_LINES;
+    h->last_slot = (int)slot;
     return DM_OK;
 }
 

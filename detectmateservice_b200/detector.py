@@ -145,7 +145,8 @@ class DeviceDetector:
 
     def collect(self, slot: int = 0) -> Tuple[np.ndarray, np.ndarray]:
         """Wait for `slot`; returns (flags, scores) as views of the handle's pinned result
-        buffers (valid until the slot is submitted again)."""
+        buffers (valid until the slot is submitted again).  The slot's batch becomes the last
+        batch: encode_alerts() words it until the next submit()."""
         pf, ps = C.c_void_p(), C.c_void_p()
         n_lines, n_anom = C.c_uint64(), C.c_uint64()
         _lib.check(self._lib.dm_collect(self._h, int(slot), C.byref(pf), C.byref(ps), C.byref(n_lines), C.byref(n_anom)))
@@ -307,9 +308,10 @@ class DeviceDetector:
             self._pin_alerts = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
 
     def encode_alerts(self, first_log_id: int, first_alert_id: int, now: int) -> Optional[Tuple[bytes, int]]:
-        """The varint-delimited DetectorSchemas of the last process_lines(), process_logs() or process_records() batch
-        (dm_encode_alerts) and their count, or None when the device declines the batch (the caller then encodes it on
-        the host).  first_log_id numbers raw lines only; LogSchema and ParserSchema alerts carry the record's logID."""
+        """The varint-delimited DetectorSchemas of the last process_lines(), process_logs(), process_records() or
+        collect() batch (dm_encode_alerts) and their count, or None when the device declines the batch (the caller then
+        encodes it on the host).  first_log_id numbers raw lines only; LogSchema and ParserSchema alerts carry the
+        record's logID.  A collected slot must be encoded before it is submitted again."""
         out_len, n, declined = C.c_uint64(), C.c_uint64(), C.c_int()
         buf = self._pin_alerts
         _lib.check(self._lib.dm_encode_alerts(self._h, int(first_log_id), int(first_alert_id), int(now), buf.data_ptr(),

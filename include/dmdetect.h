@@ -263,8 +263,9 @@ int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delim
  *                           variables[i]);
  *   time_capture          : log_format mode: the header capture whose text is the record's Time, 0xFFFFFFFF = none
  *                           (key=value mode always takes msg=audit(<Time>...), R-tok L7).
- * dm_encode_alerts encodes the last batch of dm_process_lines (whichever kernel ran it), dm_process_logs or
- * dm_process_records into `out`: one varint-length-delimited DetectorSchema per anomalous record, in record order;
+ * dm_encode_alerts encodes the last batch of dm_process_lines (whichever kernel ran it), dm_process_logs,
+ * dm_process_records or dm_collect (a slot of the pipelined path, worded as a dm_process_lines batch) into `out`: one
+ * varint-length-delimited DetectorSchema per anomalous record, in record order;
  * alertID = first_alert_id + j (signed), detectionTimestamp = receivedTimestamp = now, extractedTimestamps =
  * [int(float(Time))], or now when the record has no Time or its Time is no float literal.  logIDs = [first_log_id +
  * record index] for raw lines; the record's own logID (LogSchema field 2, ParserSchema field 8, the last one; "" when
@@ -278,8 +279,11 @@ int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delim
  * Synchronous; ends the overlap chain of dm_process_lines.  The encoder reads the batch's message, its scores and its
  * anomaly list, which the next overlapped call rewrites; so a device-resident caller must leave that call's `buf` --
  * and its `scores_out`, when it passed a device scores buffer -- unchanged until dm_encode_alerts returns, and must not
- * enqueue another dm_process_lines on the handle in between.  DM_ERR_STATE when the last batch came from another entry
- * point (dm_process_values, the pipelined path). */
+ * enqueue another dm_process_lines on the handle in between.  A collected slot is encoded on a stream that follows its
+ * kernels, while the other slot's message stays in flight; the slot's input and anomaly list must survive until the
+ * call returns, so call it after dm_collect(slot) and before the next dm_submit_lines on that slot (with two slots in
+ * turn: collect piece i, encode it, then submit piece i + 2).  DM_ERR_STATE when the last batch came from another
+ * entry point (dm_process_values, dm_parse_logs, dm_import_known) or dm_submit_lines was called since. */
 int dm_set_alert_format(dm_handle* h, uint32_t n_strings, const uint8_t* strings, const uint32_t* string_lens,
                         const uint32_t* bits_off, const uint32_t* bits, uint32_t n_combos, const uint32_t* combo_off,
                         const uint32_t* combo_members, uint32_t time_capture, uint64_t out_cap);
@@ -316,7 +320,9 @@ int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, int delimit
  * the slot is submitted again).  While slot 1's message is crossing PCIe, slot 0's kernels
  * run and its results travel back.  Messages are processed in submission order (training
  * before detection is preserved).  Raw-mode equivalent of calling dm_process_lines per
- * message; replaces the same per-record calls of core.py:201-203. */
+ * message; replaces the same per-record calls of core.py:201-203.  dm_submit_lines leaves the
+ * handle without a last batch; dm_collect makes the slot's batch the last batch, which
+ * dm_encode_alerts can then word (see there for how long the slot must stay untouched). */
 int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t nbytes, uint64_t n_train_lines, uint32_t slot);
 int dm_collect(dm_handle* h, uint32_t slot, const uint8_t** flags_out, const float** scores_out,
                uint64_t* n_lines_out, uint64_t* n_anomalies_out);
