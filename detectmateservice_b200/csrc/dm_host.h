@@ -68,6 +68,16 @@ inline uint32_t dm_anomalies_merge(dm_anomaly_t* v, uint32_t n) {
     return m;
 }
 
+// The keys a window with keys carries: novel-list entries [from, to) of the `learnt` keys this rank has learnt so far
+// (at most novel_cap are listed), of which `exported` have travelled already; at most `cap` per window, the rest
+// (`pending`) waits for the next window.  Truncating instead of failing keeps every rank in the collective.
+struct DmWindowKeys { uint64_t from, to, pending; };
+inline DmWindowKeys dm_window_keys(uint64_t exported, uint64_t learnt, uint64_t novel_cap, uint64_t cap) {
+    const uint64_t listed = std::min(learnt, novel_cap);
+    const uint64_t to = std::min(listed, exported + cap);
+    return DmWindowKeys{exported, to, listed - to};
+}
+
 // What a synchronous record call (dm_process_values, dm_process_records) adds to the statistics words on the host:
 // lines, train_lines, detect_lines and bytes.
 inline void dm_stats_add_records(unsigned long long* w, uint64_t n_records, uint64_t trained, uint64_t scored, uint64_t nbytes) {

@@ -22,6 +22,7 @@
 #include "dm_kernels_lanes.cuh"
 #include "dm_kernels_alerts.cuh"
 #include "dm_kernels_parse.cuh"
+#include "dm_kernels_window.cuh"
 #include "dm_format_host.h"
 #include "dm_host.h"
 
@@ -103,6 +104,7 @@ struct dm_handle {
     unsigned long long* d_win[2] = {nullptr, nullptr};   // window exchange buffers of dm_window_allreduce
     cudaEvent_t ev_win_done[2] = {nullptr, nullptr};
     uint64_t win_seq = 0;
+    cudaEvent_t ev_import = nullptr;     // recorded by every dm_window_import, on whichever stream it ran
     bool fmt_set = false;
     uint32_t fmt_slots = 1;        // DmFormat.max_slots (dynamic shared memory of the thread-per-record kernel)
     // LogSchema input (dm_process_logs), allocated on first use
@@ -238,6 +240,7 @@ static int dm_create_fill(dm_handle* h, int device, const cudaDeviceProp& prop, 
     h->d_stats_exported = h->d_stats + DM_STATS_WORDS;
     h->d_stats_global = h->d_stats + 2 * DM_STATS_WORDS;
     DM_CUDA(cudaHostAlloc(&h->h_stats, DM_STATS_WORDS * sizeof(unsigned long long), cudaHostAllocDefault));
+    DM_CUDA(cudaEventCreateWithFlags(&h->ev_import, cudaEventDisableTiming));
 
     const uint64_t cap = 1ull << table_log2_slots;
     h->table.mask = (uint32_t)(cap - 1);
@@ -373,6 +376,7 @@ extern "C" int dm_destroy(dm_handle* h) {
         if (sl.st_out) cudaStreamDestroy(sl.st_out);
     }
     if (h->st_in) cudaStreamDestroy(h->st_in);
+    if (h->ev_import) cudaEventDestroy(h->ev_import);
     if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
     return DM_OK;
@@ -1302,6 +1306,7 @@ extern "C" int dm_collect_anomalies(dm_handle* h, uint32_t slot, dm_anomaly_t* o
 extern "C" int dm_sync(dm_handle* h, uint64_t* n_lines_out, uint64_t* n_anomalies_out) {
     if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
     DM_CUDA(cudaSetDevice(h->device));
+    DM_CUDA(cudaStreamWaitEvent(h->last_stream, h->ev_import, 0));     // the last window import, whatever its stream
     DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, h->last_stream));
     int rc = dm_fetch_errors(h, h->last_stream);
     if (rc != DM_OK) return rc;
@@ -1345,6 +1350,7 @@ extern "C" int dm_get_stats(dm_handle* h, dm_stats_t* out) {
 extern "C" int dm_get_global_stats(dm_handle* h, dm_stats_t* out) {
     if (!h || !out) return dm_fail(DM_ERR_ARG, "NULL argument");
     DM_CUDA(cudaSetDevice(h->device));
+    DM_CUDA(cudaStreamWaitEvent(h->last_stream, h->ev_import, 0));     // the last window import, whatever its stream
     DM_CUDA(cudaStreamSynchronize(h->last_stream));
     DM_CUDA(cudaMemcpy(h->h_stats, h->d_stats_global, DM_STATS_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     dm_words_to_stats(h->h_stats, out);
@@ -1354,13 +1360,6 @@ extern "C" int dm_get_global_stats(dm_handle* h, dm_stats_t* out) {
 // ---------------------------------------------------------------------------------------
 // known-set export / import / reset
 // ---------------------------------------------------------------------------------------
-__global__ void dm_k_insert_keys(DmTable t, const unsigned long long* __restrict__ keys, uint64_t n, unsigned int* err) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-        unsigned long long k = keys[i];
-        if (k) dm_table_insert(t, k, err, false);
-    }
-}
-
 extern "C" int dm_export_known(dm_handle* h, uint64_t* keys_out, uint64_t cap, uint64_t* n_out) {
     if (!h || !n_out) return dm_fail(DM_ERR_ARG, "NULL argument");
     DM_CUDA(cudaSetDevice(h->device));
@@ -1409,54 +1408,12 @@ extern "C" int dm_reset(dm_handle* h) {
 }
 
 // ---------------------------------------------------------------------------------------
-// multi-GPU window exchange
-//   buffer layout (uint64 words): [0, DM_STATS_WORDS) statistics delta, summed over ranks;
-//   with_keys: then per rank r a segment [count, key_0 .. key_{DM_WINDOW_KEYS-1}] that only
-//   rank r fills, so the SUM all-reduce concatenates the segments.
+// multi-GPU window exchange (buffer layout and kernels: dm_kernels_window.cuh, with
+// DM_WINDOW_KEYS keys per rank segment)
 // ---------------------------------------------------------------------------------------
 extern "C" uint64_t dm_window_words(dm_handle* h, uint32_t world, int with_keys) {
     (void)h;
-    return (uint64_t)DM_STATS_WORDS + (with_keys ? (uint64_t)world * (1ull + DM_WINDOW_KEYS) : 0ull);
-}
-
-__global__ void dm_k_window_export(unsigned long long* __restrict__ out, uint64_t n_words,
-                                   unsigned long long* __restrict__ stats, unsigned long long* __restrict__ exported,
-                                   const unsigned long long* __restrict__ table_count,
-                                   const unsigned long long* __restrict__ novel, uint64_t novel_from, uint64_t novel_to,
-                                   uint64_t seg_off, int with_keys) {
-    const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const uint64_t nth = (uint64_t)gridDim.x * blockDim.x;
-    for (uint64_t i = tid; i < n_words; i += nth) {
-        unsigned long long v = 0;
-        if (i < DM_STATS_WORDS) {
-            unsigned long long cur = (i == 6) ? 0ull : stats[i];
-            v = cur - atomicExch(exported + i, cur);      // telescopes mod 2^64 whatever the order of in-flight windows
-        } else if (with_keys && i >= seg_off && i < seg_off + 1 + DM_WINDOW_KEYS) {
-            const uint64_t j = i - seg_off;
-            if (j == 0) v = novel_to - novel_from;
-            else if (novel_from + j - 1 < novel_to) v = novel[novel_from + j - 1];
-        }
-        out[i] = v;
-    }
-    (void)table_count;
-}
-
-__global__ void dm_k_window_import(const unsigned long long* __restrict__ in, uint32_t world, uint32_t self_rank,
-                                   unsigned long long* __restrict__ global_stats, DmTable t, unsigned int* err,
-                                   int with_keys) {
-    const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const uint64_t nth = (uint64_t)gridDim.x * blockDim.x;
-    if (tid < DM_STATS_WORDS) atomicAdd(global_stats + tid, in[tid]);     // (two windows may be in flight)
-    if (!with_keys) return;
-    for (uint32_t r = 0; r < world; ++r) {
-        if (r == self_rank) continue;            // own keys are already in the local table
-        const uint64_t seg = (uint64_t)DM_STATS_WORDS + (uint64_t)r * (1ull + DM_WINDOW_KEYS);
-        const uint64_t cnt = in[seg];
-        for (uint64_t j = tid; j < cnt && j < DM_WINDOW_KEYS; j += nth) {
-            unsigned long long k = in[seg + 1 + j];
-            if (k) dm_table_insert(t, k, err, false);
-        }
-    }
+    return dm_window_n_words(world, with_keys != 0, DM_WINDOW_KEYS);
 }
 
 extern "C" int dm_window_export(dm_handle* h, uint64_t* dev_buf, uint32_t rank, uint32_t world, int with_keys, void* stream_) {
@@ -1464,25 +1421,24 @@ extern "C" int dm_window_export(dm_handle* h, uint64_t* dev_buf, uint32_t rank, 
     DM_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream;     // (not recorded as the compute stream)
     dm_break_chain(h, st);
-    uint64_t novel_to = h->novel_exported;
+    DmWindowKeys wk{h->novel_exported, h->novel_exported, 0};
     if (with_keys) {
         // the number of keys learnt so far is needed on the host to bound the segment
         unsigned long long cnt[2];
         DM_CUDA(cudaMemcpyAsync(cnt, h->table.count, sizeof(cnt), cudaMemcpyDeviceToHost, st));
         DM_CUDA(cudaStreamSynchronize(st));
-        novel_to = std::min<uint64_t>(cnt[1], h->table.novel_cap);
         // at most DM_WINDOW_KEYS keys travel per window; the rest goes with the next one (dm_window_pending_keys).
         // Failing here instead would leave the other ranks waiting in the all-reduce.
-        if (novel_to - h->novel_exported > DM_WINDOW_KEYS) novel_to = h->novel_exported + DM_WINDOW_KEYS;
-        h->novel_pending = std::min<uint64_t>(cnt[1], h->table.novel_cap) - novel_to;
+        wk = dm_window_keys(h->novel_exported, cnt[1], h->table.novel_cap, DM_WINDOW_KEYS);
+        h->novel_pending = wk.pending;
     }
     const uint64_t n_words = dm_window_words(h, world, with_keys);
-    const uint64_t seg_off = (uint64_t)DM_STATS_WORDS + (uint64_t)rank * (1ull + DM_WINDOW_KEYS);
+    const uint64_t seg_off = dm_window_n_words(rank, true, DM_WINDOW_KEYS);
     dm_k_window_export<<<std::max(1, (int)std::min<uint64_t>((n_words + 255) / 256, 2048)), 256, 0, st>>>(
-        (unsigned long long*)dev_buf, n_words, h->d_stats, h->d_stats_exported, h->table.count, h->table.novel,
-        h->novel_exported, novel_to, seg_off, with_keys);
+        (unsigned long long*)dev_buf, n_words, h->d_stats, h->d_stats_exported, h->table.novel, wk.from, wk.to, seg_off,
+        DM_WINDOW_KEYS, with_keys);
     DM_CUDA(cudaGetLastError());
-    h->novel_exported = novel_to;
+    h->novel_exported = wk.to;
     return DM_OK;
 }
 
@@ -1497,10 +1453,12 @@ extern "C" int dm_window_import(dm_handle* h, const uint64_t* dev_buf, uint32_t 
     DM_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream;     // (not recorded as the compute stream)
     dm_break_chain(h, st);
-    dm_k_window_import<<<with_keys ? 256 : 1, 256, 0, st>>>((const unsigned long long*)dev_buf, world, rank,
-                                                          h->d_stats_global, h->table, &h->d_hdr->error, with_keys);
+    // errors go to the handle's accumulating error word, which no launch overwrites: the next dm_sync or synchronous
+    // dm_process_lines reports them (the batch header's word is rewritten by the next detection launch)
+    dm_k_window_import<<<with_keys ? 256 : 1, 256, 0, st>>>((const unsigned long long*)dev_buf, world, rank, DM_WINDOW_KEYS,
+                                                          h->d_stats_global, h->table, &h->dmx.d_shared->error, with_keys);
     DM_CUDA(cudaGetLastError());
-    // (keys received from peers are inserted without joining the novel list: they are not shipped again)
+    DM_CUDA(cudaEventRecord(h->ev_import, st));     // dm_sync and dm_get_global_stats wait for it
     return DM_OK;
 }
 

@@ -438,5 +438,13 @@ class DeviceDetector:
         """export + ncclAllReduce + import of one window, enqueued on `stream` by one call."""
         _lib.check(self._lib.dm_window_allreduce(self._h, int(with_keys), stream or None))
 
+    def window_pending_keys(self) -> int:
+        """After an export with keys: this rank's learnt keys that did not fit in the window (dm_window_pending_keys).
+        While any rank reports some, every rank runs another exchange with keys."""
+        n = C.c_uint64()
+        _lib.check(self._lib.dm_window_pending_keys(self._h, C.byref(n)))
+        return n.value
+
     def window_import(self, dev_ptr: int, rank: int, world: int, with_keys: bool, stream: int = 0) -> None:
+        """Its errors (a table over its load limit) are reported by the next sync() or synchronous process_lines()."""
         _lib.check(self._lib.dm_window_import(self._h, dev_ptr, rank, world, int(with_keys), stream or None))

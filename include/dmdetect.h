@@ -358,13 +358,17 @@ uint64_t dm_table_key(uint32_t field, const uint8_t* value, uint32_t len);
  * (rank r writes its keys only into segment r, so the sum is a concatenation).
  *   export : pack this rank's delta since the previous window into dev_buf (device memory).
  *   (caller all-reduces dev_buf with SUM over uint64 -- NCCL over NVLink via torch.distributed)
- *   import : insert all ranks' keys into the local table, fold the global statistics. */
+ *   import : insert all ranks' keys into the local table, fold the global statistics.
+ * Export and import run on `stream` (NULL: the handle's own).  An import with keys changes the table that detection
+ * reads: the caller orders it before any later detection on the handle (e.g. the same stream).  An import's errors
+ * (the table over its load limit) are reported by the next dm_sync or synchronous dm_process_lines. */
 uint64_t dm_window_words(dm_handle* h, uint32_t world, int with_keys);
 int dm_window_export(dm_handle* h, uint64_t* dev_buf, uint32_t rank, uint32_t world, int with_keys, void* stream);
 int dm_window_import(dm_handle* h, const uint64_t* dev_buf, uint32_t rank, uint32_t world, int with_keys, void* stream);
 /* A window carries at most 65536 newly learnt keys per rank.  After an export with keys: how many of this rank's
  * learnt keys are still waiting (0 in all but pathological training windows).  When any rank reports > 0 the caller
- * runs another exchange with keys before detection starts (all ranks call the collective the same number of times). */
+ * runs another exchange with keys before detection starts (all ranks call the collective the same number of times);
+ * window.DeviceWindow.exchange does so.  dm_window_allreduce's export sets the count too. */
 int dm_window_pending_keys(dm_handle* h, uint64_t* n_out);
 
 /* The same exchange done by the library itself: export, ncclAllReduce(sum, uint64) over the
@@ -378,7 +382,8 @@ int dm_window_pending_keys(dm_handle* h, uint64_t* n_out);
 int dm_nccl_unique_id(uint8_t* out128);
 int dm_nccl_init(dm_handle* h, const uint8_t* ids, uint32_t n_comms, uint32_t rank, uint32_t world);
 int dm_window_allreduce(dm_handle* h, int with_keys, void* stream);
-/* Statistics summed over all ranks as of the last dm_window_import. */
+/* Statistics summed over all ranks as of the last dm_window_import, whatever stream it was enqueued on (this call and
+ * dm_sync wait for it). */
 int dm_get_global_stats(dm_handle* h, dm_stats_t* out);
 
 /* Measurement support (bench.py): when enabled, every dm_process_lines records a CUDA

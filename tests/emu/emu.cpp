@@ -21,6 +21,7 @@
 #include "dm_kernels_logs.cuh"
 #include "dm_kernels_alerts.cuh"
 #include "dm_kernels_parse.cuh"
+#include "dm_kernels_window.cuh"
 #include "dm_format_host.h"
 #include "dm_host.h"
 
@@ -64,6 +65,9 @@ struct EmuHandle {
     std::vector<unsigned long long> slots, novel;
     unsigned long long counts[2] = {0, 0};
     unsigned long long stats[DM_STATS_WORDS] = {0};
+    unsigned long long stats_exported[DM_STATS_WORDS] = {0};   // the window exchange (dm_handle::d_stats_exported,
+    unsigned long long stats_global[DM_STATS_WORDS] = {0};     //   d_stats_global, novel_exported, novel_pending)
+    uint64_t novel_exported = 0, novel_pending = 0;
     DmBatchHeader hdr;
     std::vector<dm_anomaly_t> anoms;
     uint64_t max_lines = 0;
@@ -717,10 +721,58 @@ extern "C" void emu_get_stats(EmuHandle* h, unsigned long long* out) {
     out[6] = h->counts[0];
 }
 
+// as dm_export_known: every key of the table (own records, peers, emu_import_known), sorted; their count
 extern "C" uint64_t emu_export_known(EmuHandle* h, unsigned long long* out, uint64_t cap) {
-    uint64_t n = std::min<uint64_t>(h->counts[1], h->novel.size());
-    std::vector<unsigned long long> v(h->novel.begin(), h->novel.begin() + n);
+    std::vector<unsigned long long> v;
+    for (unsigned long long k : h->slots)
+        if (k) v.push_back(k);
     std::sort(v.begin(), v.end());
-    for (uint64_t i = 0; i < n && i < cap; ++i) out[i] = v[i];
-    return n;
+    for (uint64_t i = 0; i < v.size() && i < cap; ++i) out[i] = v[i];
+    return v.size();
+}
+
+// as dm_import_known (dm_k_insert_keys on 2 CTAs of 32 threads); the error bits
+extern "C" uint32_t emu_import_known(EmuHandle* h, const unsigned long long* keys, uint64_t n) {
+    unsigned int err = 0;
+    if (n) emu_launch_grid(2, 32, [&] { dm_k_insert_keys(h->table, keys, n, &err); });
+    return err;
+}
+
+// ---------------------------------------------------------------------------------------------- window exchange
+// As dm_window_words / dm_window_export / dm_window_import / dm_window_pending_keys with seg_keys keys per rank segment
+// (libdmdetect: DM_WINDOW_KEYS).  The kernels run on 2 CTAs of 32 threads, so that both take their stride loops.
+extern "C" uint64_t emu_window_words(uint32_t world, int with_keys, uint64_t seg_keys) {
+    return dm_window_n_words(world, with_keys != 0, seg_keys);
+}
+
+extern "C" void emu_window_export(EmuHandle* h, unsigned long long* buf, uint32_t rank, uint32_t world, int with_keys,
+                                  uint64_t seg_keys) {
+    DmWindowKeys wk{h->novel_exported, h->novel_exported, 0};
+    if (with_keys) {
+        wk = dm_window_keys(h->novel_exported, h->counts[1], h->table.novel_cap, seg_keys);
+        h->novel_pending = wk.pending;
+    }
+    const uint64_t n_words = dm_window_n_words(world, with_keys != 0, seg_keys);
+    const uint64_t seg_off = dm_window_n_words(rank, true, seg_keys);
+    emu_launch_grid(2, 32, [&] {
+        dm_k_window_export(buf, n_words, h->stats, h->stats_exported, h->novel.data(), wk.from, wk.to, seg_off, seg_keys,
+                           with_keys);
+    });
+    h->novel_exported = wk.to;
+}
+
+extern "C" uint64_t emu_window_pending_keys(EmuHandle* h) { return h->novel_pending; }
+
+// the error bits the import leaves in the handle's error word (dm_sync reports them)
+extern "C" uint32_t emu_window_import(EmuHandle* h, const unsigned long long* buf, uint32_t rank, uint32_t world,
+                                      int with_keys, uint64_t seg_keys) {
+    unsigned int err = 0;
+    emu_launch_grid(2, 32, [&] {
+        dm_k_window_import(buf, world, rank, seg_keys, h->stats_global, h->table, &err, with_keys);
+    });
+    return err;
+}
+
+extern "C" void emu_get_global_stats(EmuHandle* h, unsigned long long* out) {
+    for (int i = 0; i < DM_STATS_WORDS; ++i) out[i] = h->stats_global[i];
 }

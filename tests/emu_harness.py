@@ -71,6 +71,12 @@ _SIGNATURES = {                                                   # name: (resty
     "emu_get_anomalies": (C.c_uint32, [C.c_void_p, C.POINTER(Anomaly), C.c_uint32]),
     "emu_get_stats": (None, [C.c_void_p, _P64]),
     "emu_export_known": (C.c_uint64, [C.c_void_p, _P64, C.c_uint64]),
+    "emu_import_known": (C.c_uint32, [C.c_void_p, C.c_void_p, C.c_uint64]),
+    "emu_window_words": (C.c_uint64, [C.c_uint32, C.c_int, C.c_uint64]),
+    "emu_window_export": (None, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.c_uint64]),
+    "emu_window_pending_keys": (C.c_uint64, [C.c_void_p]),
+    "emu_window_import": (C.c_uint32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.c_uint64]),
+    "emu_get_global_stats": (None, [C.c_void_p, _P64]),
 }
 
 
@@ -99,6 +105,7 @@ class EmuDetector:
         self.h = self.lib.emu_create(len(self.keys), b"".join(self.keys), lens, table_log2,
                                      max_bytes // TILE_BYTES + 2, max_lines)
         self.max_lines = max_lines
+        self.table_log2 = table_log2
 
     def close(self):
         if self.h:
@@ -156,13 +163,45 @@ class EmuDetector:
         n = self.lib.emu_get_anomalies(self.h, arr, 65536)
         return [(arr[i].line, arr[i].mask, arr[i].offset) for i in range(n)]
 
-    def stats(self):
+    def _stats(self, fn):
         w = (C.c_uint64 * 40)()
-        self.lib.emu_get_stats(self.h, w)
+        fn(self.h, w)
         return {"lines": w[0], "train_lines": w[1], "detect_lines": w[2], "anomalies": w[3], "score_sum": w[4],
                 "bytes": w[5], "known_keys": w[6], "bad_records": w[7], "unknown_per_key": [w[8 + i] for i in range(len(self.keys))]}
 
+    def stats(self):
+        return self._stats(self.lib.emu_get_stats)
+
+    def global_stats(self):
+        """The statistics summed over the ranks by the window imports so far (dm_get_global_stats)."""
+        return self._stats(self.lib.emu_get_global_stats)
+
     def export_known(self):
-        out = (C.c_uint64 * (1 << 16))()
-        n = self.lib.emu_export_known(self.h, out, 1 << 16)
+        """Every key of the table, sorted (dm_export_known)."""
+        out = (C.c_uint64 * (1 << self.table_log2))()
+        n = self.lib.emu_export_known(self.h, out, 1 << self.table_log2)
         return [out[i] for i in range(n)]
+
+    def import_known(self, keys):
+        """dm_import_known; returns the DM_DEVERR_* bits of the insert."""
+        a = np.ascontiguousarray(keys, dtype=np.uint64)
+        return self.lib.emu_import_known(self.h, a.ctypes.data, a.size)
+
+    # the window exchange, seg_keys keys per rank segment (libdmdetect: 65536); buffers are uint64 numpy arrays
+    def window_words(self, world, with_keys, seg_keys):
+        return int(self.lib.emu_window_words(world, int(with_keys), seg_keys))
+
+    def window_export(self, rank, world, with_keys, seg_keys):
+        """dm_window_export into a fresh buffer filled with hostile words first; the buffer."""
+        buf = np.full(self.window_words(world, with_keys, seg_keys), 0xDEADBEEFDEADBEEF, dtype=np.uint64)
+        self.lib.emu_window_export(self.h, buf.ctypes.data, rank, world, int(with_keys), seg_keys)
+        return buf
+
+    def window_pending_keys(self):
+        return int(self.lib.emu_window_pending_keys(self.h))
+
+    def window_import(self, buf, rank, world, with_keys, seg_keys):
+        """dm_window_import of an all-reduced buffer; returns the DM_DEVERR_* bits it leaves for the next sync."""
+        a = np.ascontiguousarray(buf).view(np.uint64)
+        assert a.size == self.window_words(world, with_keys, seg_keys)
+        return self.lib.emu_window_import(self.h, a.ctypes.data, rank, world, int(with_keys), seg_keys)
