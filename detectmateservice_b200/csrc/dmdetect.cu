@@ -105,6 +105,7 @@ struct dm_handle {
     cudaEvent_t ev_win_done[2] = {nullptr, nullptr};
     uint64_t win_seq = 0;
     cudaEvent_t ev_import = nullptr;     // recorded by every dm_window_import, on whichever stream it ran
+    cudaEvent_t ev_order = nullptr;      // dm_use_stream: the previous stream's work, waited for by the next stream
     bool fmt_set = false;
     uint32_t fmt_slots = 1;        // DmFormat.max_slots (dynamic shared memory of the thread-per-record kernel)
     // LogSchema input (dm_process_logs), allocated on first use
@@ -177,16 +178,28 @@ static void dm_prof_mark_cb(void* ctx, cudaStream_t st, int which) { dm_prof_mar
 
 static const uint32_t DM_WINDOW_KEYS = 1u << 16;    // keys one rank can ship per window
 
-static int dm_pick_stream(dm_handle* h, void* stream, cudaStream_t* out) {
-    *out = stream ? (cudaStream_t)stream : h->stream;
-    h->last_stream = *out;
-    return DM_OK;
-}
-
 // Anything this library enqueues that is not a stream-variant detect launch ends the chain of
 // overlapping launches on that stream: the next detect launch is then ordered behind it in full.
 static void dm_break_chain(dm_handle* h, cudaStream_t st) {
     if (h->dmx.chain_stream == st) h->dmx.chain_stream = nullptr;
+}
+
+// Makes st the stream of the handle's next enqueue.  A call on another stream than the previous one first waits for
+// the previous stream, and so for every earlier call: the handle's calls take effect in call order whatever streams
+// they use, and waiting for last_stream waits for everything the handle enqueued.  A switch also ends the overlap
+// chain.  Calls on one stream record and wait on nothing.
+static int dm_use_stream(dm_handle* h, cudaStream_t st) {
+    if (st == h->last_stream) return DM_OK;
+    DM_CUDA(cudaEventRecord(h->ev_order, h->last_stream));
+    DM_CUDA(cudaStreamWaitEvent(st, h->ev_order, 0));
+    h->last_stream = st;
+    h->dmx.chain_stream = nullptr;
+    return DM_OK;
+}
+
+static int dm_pick_stream(dm_handle* h, void* stream, cudaStream_t* out) {
+    *out = stream ? (cudaStream_t)stream : h->stream;
+    return dm_use_stream(h, *out);
 }
 
 extern "C" int dm_destroy(dm_handle* h);
@@ -241,6 +254,7 @@ static int dm_create_fill(dm_handle* h, int device, const cudaDeviceProp& prop, 
     h->d_stats_global = h->d_stats + 2 * DM_STATS_WORDS;
     DM_CUDA(cudaHostAlloc(&h->h_stats, DM_STATS_WORDS * sizeof(unsigned long long), cudaHostAllocDefault));
     DM_CUDA(cudaEventCreateWithFlags(&h->ev_import, cudaEventDisableTiming));
+    DM_CUDA(cudaEventCreateWithFlags(&h->ev_order, cudaEventDisableTiming));
 
     const uint64_t cap = 1ull << table_log2_slots;
     h->table.mask = (uint32_t)(cap - 1);
@@ -377,6 +391,7 @@ extern "C" int dm_destroy(dm_handle* h) {
     }
     if (h->st_in) cudaStreamDestroy(h->st_in);
     if (h->ev_import) cudaEventDestroy(h->ev_import);
+    if (h->ev_order) cudaEventDestroy(h->ev_order);
     if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
     return DM_OK;
@@ -425,7 +440,8 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     if (buf_on_device && (((uintptr_t)buf) & 15)) return dm_fail(DM_ERR_ARG, "device buf must be 16-byte aligned");
     DM_CUDA(cudaSetDevice(h->device));
     cudaStream_t st;
-    dm_pick_stream(h, stream_, &st);
+    const int rc_st = dm_pick_stream(h, stream_, &st);
+    if (rc_st != DM_OK) return rc_st;
 
     const uint8_t* d_buf = buf;
     if (!buf_on_device) {
@@ -518,13 +534,17 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
 // ---------------------------------------------------------------------------------------
 // record mode
 // ---------------------------------------------------------------------------------------
-// Adds what a synchronous record call counts on the host (dm_stats_add_records) to the handle's statistics.
-static int dm_records_stats(dm_handle* h, uint64_t n_records, uint64_t trained, uint64_t scored, uint64_t nbytes) {
+// Adds what a synchronous record call counts on the host (dm_stats_add_records) to the handle's statistics.  The
+// read-modify-write runs on the call's stream st: a copy on the legacy stream is not ordered against the handle's
+// non-blocking streams, so a later kernel could add to d_stats before the write-back lands.
+static int dm_records_stats(dm_handle* h, cudaStream_t st, uint64_t n_records, uint64_t trained, uint64_t scored, uint64_t nbytes) {
     unsigned long long cur[6];
-    DM_CUDA(cudaMemcpy(cur, h->d_stats, sizeof(cur), cudaMemcpyDeviceToHost));
+    DM_CUDA(cudaMemcpyAsync(cur, h->d_stats, sizeof(cur), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
     dm_stats_add_records(cur, n_records, trained, scored, nbytes);
-    DM_CUDA(cudaMemcpy(h->d_stats, cur, 3 * sizeof(cur[0]), cudaMemcpyHostToDevice));
-    DM_CUDA(cudaMemcpy(h->d_stats + 5, &cur[5], sizeof(cur[5]), cudaMemcpyHostToDevice));
+    DM_CUDA(cudaMemcpyAsync(h->d_stats, cur, 3 * sizeof(cur[0]), cudaMemcpyHostToDevice, st));
+    DM_CUDA(cudaMemcpyAsync(h->d_stats + 5, &cur[5], sizeof(cur[5]), cudaMemcpyHostToDevice, st));
+    DM_CUDA(cudaStreamSynchronize(st));
     return DM_OK;
 }
 
@@ -544,7 +564,8 @@ extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blo
     }
     DM_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
-    h->last_stream = st;
+    int rc = dm_use_stream(h, st);
+    if (rc != DM_OK) return rc;
     dm_break_chain(h, st);
     h->last_src = DMA_SRC_NONE;
     if (n_values > h->vals_cap) {
@@ -586,7 +607,7 @@ extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blo
     DM_CUDA(cudaStreamSynchronize(st));
     // statistics that do not need the device: record and byte counts
     const uint32_t tr = std::min<uint32_t>(n_train_records, n_records);
-    int rc = dm_records_stats(h, n_records, tr, n_records - tr, record_bytes);
+    rc = dm_records_stats(h, st, n_records, tr, n_records - tr, record_bytes);
     if (rc != DM_OK) return rc;
     h->h_hdr->n_lines = n_records;
     rc = dm_check_device_errors(h);
@@ -742,7 +763,8 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
         return dm_fail(DM_ERR_CAPACITY, "batch holds %u records, output capacity is %llu", n_records, (unsigned long long)out_cap);
     DM_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
-    h->last_stream = st;
+    int rc = dm_use_stream(h, st);
+    if (rc != DM_OK) return rc;
     dm_break_chain(h, st);
     h->last_src = DMA_SRC_NONE;
     if (2ull * n_records + 2 > 3ull * h->vals_cap + 1) {
@@ -790,7 +812,7 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     DM_CUDA(cudaStreamSynchronize(st));
     // train_lines: the records trained; detect_lines: the records from the bound on (malformed ones included)
     const uint64_t first_scored = n_train_records > 0 ? bound[0] : 0;
-    int rc = dm_records_stats(h, n_records, bound[1], n_records - first_scored, nbytes);
+    rc = dm_records_stats(h, st, n_records, bound[1], n_records - first_scored, nbytes);
     if (rc != DM_OK) return rc;
     h->h_hdr->n_lines = n_records;
     rc = dm_check_device_errors(h);
@@ -844,11 +866,12 @@ static int dm_logs_unwrap(dm_handle* h, const uint8_t* buf, uint64_t nbytes, con
     const uint32_t n_records = (uint32_t)fr.off.size();
     DM_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
-    h->last_stream = st;
+    int rc = dm_use_stream(h, st);
+    if (rc != DM_OK) return rc;
     dm_break_chain(h, st);
     // walk grid: at most 4 CTAs per SM
     const uint32_t walk_ctas = (uint32_t)h->sm_count * 4;
-    int rc = dm_logs_reserve(h, n_records, walk_ctas);
+    rc = dm_logs_reserve(h, n_records, walk_ctas);
     if (rc != DM_OK) return rc;
     DmLogsArgs a = dm_logs_carve(h->d_logs, h->logs_cap, h->logs_chunks, h->d_lhdr, d_rscores, d_rflags);
     dm_logs_call(&a, h->d_in, n_records, n_train_records, walk_ctas, copy ? h->d_logs_text : nullptr,
@@ -1234,7 +1257,8 @@ extern "C" int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t n
     h->slot_nbytes[slot] = nbytes;
     DM_CUDA(cudaEventRecord(sl.ev_in, h->st_in));
     cudaStream_t st = h->stream;                       // ONE compute stream: submission order = processing order
-    h->last_stream = st;
+    rc = dm_use_stream(h, st);
+    if (rc != DM_OK) return rc;
     h->last_src = DMA_SRC_NONE;
     DM_CUDA(cudaStreamWaitEvent(st, sl.ev_in, 0));
     if (nbytes == 0) DM_CUDA(cudaMemsetAsync(sl.d_hdr, 0, sizeof(DmBatchHeader), st));
@@ -1397,11 +1421,15 @@ extern "C" int dm_import_known(dm_handle* h, const uint64_t* keys, uint64_t n) {
 extern "C" int dm_reset(dm_handle* h) {
     if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
     DM_CUDA(cudaSetDevice(h->device));
-    DM_CUDA(cudaStreamSynchronize(h->last_stream));
-    DM_CUDA(cudaMemset(h->table.slots, 0, ((uint64_t)h->table.mask + 1) * sizeof(unsigned long long)));
-    DM_CUDA(cudaMemset(h->table.count, 0, 2 * sizeof(unsigned long long)));
-    DM_CUDA(cudaMemset(h->d_stats, 0, 3 * DM_STATS_WORDS * sizeof(unsigned long long)));
-    DM_CUDA(cudaMemset(h->d_hdr, 0, sizeof(DmBatchHeader)));
+    // on last_stream, behind everything the handle enqueued: a memset on the legacy stream would not order against the
+    // handle's non-blocking streams, and the next call's kernels could read the table before it is cleared
+    cudaStream_t st = h->last_stream;
+    dm_break_chain(h, st);
+    DM_CUDA(cudaMemsetAsync(h->table.slots, 0, ((uint64_t)h->table.mask + 1) * sizeof(unsigned long long), st));
+    DM_CUDA(cudaMemsetAsync(h->table.count, 0, 2 * sizeof(unsigned long long), st));
+    DM_CUDA(cudaMemsetAsync(h->d_stats, 0, 3 * DM_STATS_WORDS * sizeof(unsigned long long), st));
+    DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+    DM_CUDA(cudaStreamSynchronize(st));
     h->novel_exported = 0;
     h->novel_pending = 0;
     return DM_OK;

@@ -98,6 +98,13 @@ int dm_destroy(dm_handle* h);
  *                      returns without synchronising (device-resident pipelines; its errors are reported by
  *                      the next dm_sync or synchronous call); otherwise it returns after the results are
  *                      complete.
+ * Call order: a handle's calls take effect in the order they are made, whatever stream each one uses (`stream` here,
+ * the handle's own stream for the other entry points).  A call on another stream than the handle's previous call
+ * first waits, on the device, for that stream, so it sees the known-set table, statistics and errors of every earlier
+ * call; calls that stay on one stream add no waits.  Two kinds of call keep the ordering documented with them: the
+ * window calls (dm_window_export / _import / _allreduce), which the caller orders, so that two all-reduces can be in
+ * flight; and dm_encode_alerts of a collected slot, which is ordered behind that slot only, so that the other slot
+ * stays in flight.
  * By default a call is ordered behind everything enqueued on `stream` before it.  After
  * dm_set_overlap(h, 1) consecutive device-resident detection calls on one stream overlap
  * (programmatic dependent launch): a call may then start READING its `buf` and the known-set
@@ -329,7 +336,8 @@ int dm_collect(dm_handle* h, uint32_t slot, const uint8_t** flags_out, const flo
 /* Anomalous records of the batch last collected from `slot` (same format as dm_get_anomalies). */
 int dm_collect_anomalies(dm_handle* h, uint32_t slot, dm_anomaly_t* out, uint32_t cap, uint32_t* n_out);
 
-/* Wait for everything enqueued on the handle and report the last batch's counts.  On the default key=value kernel
+/* Wait for everything enqueued on the handle, whatever streams it went to (see "Call order" at dm_process_lines; of the
+ * window calls, the last dm_window_import), and report the last batch's counts.  On the default key=value kernel
  * the error reported is that of ANY dm_process_lines call since the last dm_sync or synchronous dm_process_lines (a
  * message with more records than out_cap_lines or max_lines, a training message that filled the known-set table, an
  * anomaly list that overflowed), not only of the last one: an enqueued message whose outputs are wrong or truncated
