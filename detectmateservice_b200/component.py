@@ -40,18 +40,29 @@ batch the device declines and single ParserSchema records of B200NewValueDetecto
 
 All detection decisions are taken on the device; there is no CPU path (DeviceDetector
 raises without a GPU).
+
+Learnt state across restarts (``params.state_path``, absent by default, rule R-state in DESIGN.md): the known-set
+table's keys and the counters n_seen / n_alerts are written to that file (state.py) after the message that ends the
+training window, on close(), at interpreter exit while a device handle is live, and after reset_state(), import_state()
+and a reconfigure() that keeps the device configuration.  At construction a file whose key_signature and key_probe
+match is restored: the counters at once, the keys into the device handle when it is created.  Nothing is saved per
+message: after an exit that runs no Python exit handler (SIGKILL, a power loss) the state is that of the last save,
+and alert IDs issued since then may be issued again.
 """
 from __future__ import annotations
 
+import logging
 import os
 import struct
 import threading
 import time
+import weakref
 from typing import Any, Dict, List, Optional, Tuple
 
 import numpy as np
 
 from . import alerts as _alerts
+from . import state as _state
 from . import wire
 from .compat import install_shims
 
@@ -59,6 +70,7 @@ install_shims()
 from detectmatelibrary.common.core import CoreComponent, CoreConfig  # noqa: E402
 
 _FORBIDDEN = (0x20, 0x22, 0x27, 0x3D, 0x0A)
+_log = logging.getLogger(__name__)
 
 
 class B200NewValueDetectorConfig(CoreConfig):
@@ -127,6 +139,23 @@ def parse_monitors(cfg: dict) -> List[Monitor]:
     return mons
 
 
+def key_signature(c) -> dict:
+    """Everything a known-set table key of component c depends on, as JSON values: the ordered monitors (event scope,
+    source, position, device key), the combinations, and the log_format with its templates, content capture and R-norm
+    flags.  The device geometry (device, max_batch_bytes, table_log2_slots) changes no key and is not part of it."""
+    lf = c.logformat
+    return {"monitors": [[m.event_id, m.source, m.pos, m.key.hex()] for m in c.monitors],
+            "combos": getattr(c, "combos", None),
+            "log_format": None if lf is None else lf.source,
+            "templates": None if lf is None else [bytes(t).hex() for t in lf.template_sources],
+            "content_name": None if lf is None else lf.content_name,
+            "norm_flags": None if lf is None else lf.flags}
+
+
+def device_geometry(c) -> tuple:
+    return (c.device, c.max_batch_bytes, c.table_log2_slots)
+
+
 # log_schema / log_schema_batch are opt-in: protobuf's runtime parses any LogSchema as a ParserSchema (the string fields
 # 1, 2, 3 and 5 are ParserSchema strings too), so `auto` cannot tell the two apart and keeps reading ParserSchema.
 INPUT_FORMATS = ("auto", "raw_lines", "parser_schema", "parser_schema_batch", "log_schema", "log_schema_batch")
@@ -135,7 +164,8 @@ INPUT_FORMATS = ("auto", "raw_lines", "parser_schema", "parser_schema_batch", "l
 class B200NewValueDetector(CoreComponent):
     accepts_bytes_like = True      # process() takes bytes, bytearray or memoryview (see service.py)
 
-    def __init__(self, name: str = "B200NewValueDetector", config: Optional[Any] = None) -> None:
+    def __init__(self, name: str = "B200NewValueDetector", config: Optional[Any] = None,
+                 _restore_state: bool = True) -> None:
         raw_cfg = config.model_dump() if hasattr(config, "model_dump") else config
         cfg = select_component_config(raw_cfg, name)
         super().__init__(name=name, config=B200NewValueDetectorConfig(
@@ -179,6 +209,13 @@ class B200NewValueDetector(CoreComponent):
         self.n_alerts = 0
         self.clock = time.time
         self._alert_sig = None                 # (handle, detector_id, method_type) the device's alert format was set for
+        self.state_path = str(cfg["state_path"]) if cfg.get("state_path") else None
+        self._state_lock = threading.RLock()   # held by process() and by every save
+        self._pending_keys = None              # restored keys, imported when the device handle is created
+        self._state_hold = False               # a reconfigure() rebuilt: no save until the new training window ends
+        self._finalizer = None                 # saves at interpreter exit while a handle is live
+        if _restore_state:
+            self._restore_state()
 
     # ------------------------------------------------------------------ device handle
     @property
@@ -192,7 +229,13 @@ class B200NewValueDetector(CoreComponent):
             if self.logformat is not None:
                 lf = self.logformat
                 self._det.set_format(lf.source, lf.template_sources, lf.content_name, lf.flags)
+            self._configure_device(self._det)
+            if self.state_path:
+                self._device_restored()
         return self._det
+
+    def _configure_device(self, det) -> None:
+        """Configuration a subclass adds to a new device handle."""
 
     # ------------------------------------------------------------------ receive buffers (lent to the transport)
     FRAME_SLOTS = 4
@@ -244,9 +287,18 @@ class B200NewValueDetector(CoreComponent):
                     return
 
     def close(self) -> None:
+        with self._state_lock:
+            if self._det is not None:
+                self._save_logged("close()")
+            self._drop_device()
+
+    def _drop_device(self) -> None:
         if self._det is not None:
             self._det.close()
             self._det = None
+        if self._finalizer is not None:
+            self._finalizer.detach()
+            self._finalizer = None
         self._alert_sig = None
 
     def reconfigure(self, config: Optional[Any]) -> bool:
@@ -258,26 +310,44 @@ class B200NewValueDetector(CoreComponent):
         on the next message: table keys are salted by the monitor's position, so the learnt state cannot be carried
         over and training starts again (n_seen = 0).  Returns True if the device configuration was rebuilt.
         Call it from the thread that calls process()."""
-        new = type(self)(name=self.name, config=config)
-        sig = lambda c: ([(m.event_id, m.source, m.pos, m.key) for m in c.monitors],
-                         None if c.logformat is None else (c.logformat.source, c.logformat.template_sources,
-                                                           c.logformat.content_name, c.logformat.flags),
-                         c.device, c.max_batch_bytes, c.table_log2_slots, getattr(c, "combos", None))
-        rebuild = sig(new) != sig(self)
-        keep = ("_det", "_frames", "_frame_lock", "n_seen", "n_alerts", "clock")
-        for k, v in vars(new).items():
-            if k not in keep:
-                setattr(self, k, v)
-        if rebuild:
-            self.close()
-            self.n_seen = 0
-            if self._frames and new.max_batch_bytes > len(self._frames[0][1]) - 64:
-                with self._frame_lock:
-                    self._frames = None                          # re-created at the new size on the next alloc_frame()
+        new = type(self)(name=self.name, config=config, _restore_state=False)
+        rebuild = key_signature(new) != key_signature(self) or device_geometry(new) != device_geometry(self)
+        keep = ("_det", "_frames", "_frame_lock", "n_seen", "n_alerts", "clock", "_state_lock", "_pending_keys",
+                "_state_hold", "_finalizer")
+        with self._state_lock:
+            if rebuild:
+                # the state file keeps the old configuration's state until the new training window ends: a restart with
+                # the old configuration (this one is not persisted by the service) still finds it
+                self._state_hold = True
+                self._pending_keys = None
+            for k, v in vars(new).items():
+                if k not in keep:
+                    setattr(self, k, v)
+            if rebuild:
+                self._drop_device()
+                self.n_seen = 0
+                if self._frames and new.max_batch_bytes > len(self._frames[0][1]) - 64:
+                    with self._frame_lock:
+                        self._frames = None                      # re-created at the new size on the next alloc_frame()
+            else:
+                self._save_logged("reconfigure()")
         return rebuild
 
     # ------------------------------------------------------------------ the plugin entry point
     def process(self, data: bytes) -> Optional[bytes]:
+        if not self.state_path:
+            return self._process(data)
+        with self._state_lock:
+            seen = self.n_seen
+            try:
+                return self._process(data)
+            finally:
+                # the message that ended the training window, a dropped one (DM_ERR_TABLE_FULL) included
+                if seen < self.data_use_training <= self.n_seen:
+                    self._state_hold = False
+                    self._save_logged("the end of training")
+
+    def _process(self, data: bytes) -> Optional[bytes]:
         if not data:
             return None
         fmt = self.input_format
@@ -690,14 +760,85 @@ class B200NewValueDetector(CoreComponent):
 
     def reset_state(self) -> None:
         """Forget everything learnt and restart the training window."""
-        self.det.reset()
-        self.n_seen = 0
-        self.n_alerts = 0
+        with self._state_lock:
+            self.det.reset()
+            self.n_seen = 0
+            self.n_alerts = 0
+            self._save_logged("reset_state()")
 
     def import_state(self, state: dict) -> None:
-        self.det.import_known(np.array(state.get("known", []), dtype=np.uint64))
-        self.n_seen = int(state.get("n_seen", 0))
-        self.n_alerts = int(state.get("n_alerts", 0))
+        with self._state_lock:
+            self.det.import_known(np.array(state.get("known", []), dtype=np.uint64))
+            self.n_seen = int(state.get("n_seen", 0))
+            self.n_alerts = int(state.get("n_alerts", 0))
+            self._save_logged("import_state()")
+
+    # ------------------------------------------------------------------ the state file (params.state_path)
+    def _state_header(self) -> dict:
+        return {"component": type(self).__name__, "key_signature": key_signature(self),
+                "key_probe": _state.probe_key(), "n_seen": int(self.n_seen), "n_alerts": int(self.n_alerts)}
+
+    def _restore_state(self) -> None:
+        """Read params.state_path if it exists (ValueError if it is not a valid state file).  A file of this component
+        class, key signature and key fingerprint restores n_seen and n_alerts now and its keys when the device handle is
+        created; any other is ignored with a warning, and replaced at the next save."""
+        if not self.state_path or not os.path.exists(self.state_path):
+            return
+        hdr, keys = _state.read_state(self.state_path)
+        want = self._state_header()
+        for field in ("component", "key_signature", "key_probe"):
+            if hdr[field] != want[field]:
+                _log.warning("%s: state file %s was written for another %s; ignored, training starts from scratch "
+                             "and the file is replaced at the next save", self.name, self.state_path, field)
+                return
+        self.n_seen = hdr["n_seen"]
+        self.n_alerts = hdr["n_alerts"]
+        self._pending_keys = keys
+
+    def _device_restored(self) -> None:
+        """A new device handle: import the restored keys, and save at interpreter exit while the handle is live."""
+        keys, self._pending_keys = self._pending_keys, None
+        if keys is not None and keys.size:
+            from ._lib import DM_ERR_TABLE_FULL
+            try:
+                self._det.import_known(keys)
+            except Exception as e:
+                if getattr(e, "code", None) != DM_ERR_TABLE_FULL:
+                    raise
+                _log.warning("%s: the %d restored keys take the table past its load limit; raise table_log2_slots",
+                             self.name, keys.size)
+        if self._finalizer is None:
+            self._finalizer = weakref.finalize(self, _save_at_exit, weakref.ref(self))
+
+    def save_state(self) -> bool:
+        """Write the learnt keys and counters to params.state_path now.  Returns False when there is nothing to write: no
+        state_path, no device handle, or a reconfigure() rebuilt the device configuration and its training window has
+        not ended.  Raises what the write raises; the previous file is then left as it was."""
+        with self._state_lock:
+            if not self.state_path or self._det is None:
+                return False
+            if self._state_hold and self.n_seen < self.data_use_training:
+                return False
+            _state.write_state(self.state_path, self._state_header(), self._det.export_known())
+            return True
+
+    def _save_logged(self, when: str) -> None:
+        if not self.state_path:
+            return
+        try:
+            self.save_state()
+        except Exception:
+            _log.exception("%s: saving the detector state to %s at %s failed", self.name, self.state_path, when)
+
+
+def _save_at_exit(ref) -> None:
+    comp = ref()
+    if comp is None or not comp._state_lock.acquire(timeout=30.0):
+        return
+    try:
+        comp._save_logged("interpreter exit")
+    finally:
+        comp._state_lock.release()
 
 
 class B200NewValueComboDetectorConfig(B200NewValueDetectorConfig):
@@ -760,23 +901,21 @@ class B200NewValueComboDetector(B200NewValueDetector):
     combination may mix header captures and the variables of its event's template.  A tuple
     has the same key in all three, so known sets carry over (export_state / import_state)."""
 
-    def __init__(self, name: str = "B200NewValueComboDetector", config: Optional[Any] = None) -> None:
+    def __init__(self, name: str = "B200NewValueComboDetector", config: Optional[Any] = None,
+                 _restore_state: bool = True) -> None:
         raw_cfg = config.model_dump() if hasattr(config, "model_dump") else config
         cfg = select_component_config(raw_cfg, name, fallback="NewValueComboDetector")
         cfg.setdefault("method_type", "new_value_combo_detector")
         cfg.setdefault("detector_id", "NewValueComboDetector" if name.startswith("B200") else name)
-        super().__init__(name=name, config={"detectors": {name: cfg}})
+        super().__init__(name=name, config={"detectors": {name: cfg}}, _restore_state=False)
         self.monitors, self.combos = parse_combos(cfg)
         if self.logformat is not None:
             check_format_combos(cfg, self.logformat)
+        if _restore_state:
+            self._restore_state()
 
-    @property
-    def det(self):
-        fresh = self._det is None
-        d = B200NewValueDetector.det.fget(self)
-        if fresh:
-            d.set_combos(self.combos, member_only_mask=(1 << len(self.monitors)) - 1)
-        return d
+    def _configure_device(self, det) -> None:
+        det.set_combos(self.combos, member_only_mask=(1 << len(self.monitors)) - 1)
 
     def _description(self) -> str:
         return f"{self.detector_id} detects value combinations not encountered in training as anomalies."

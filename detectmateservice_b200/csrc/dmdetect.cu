@@ -162,6 +162,10 @@ struct dm_handle {
     // last_buf is that slot's input; every other call that makes or clears a last batch changes one of the two.
     int last_slot = -1;
     uint64_t slot_nbytes[2] = {0, 0};    // the message each slot was submitted last
+    // dm_export_known's scratch (dm_known_scratch), allocated by the first export that finds a key
+    void* known_buf = nullptr;
+    DmKnownScratch known{};
+    unsigned int* h_known_hist = nullptr;   // pinned: the digit histograms and the compacted count
 };
 
 static const size_t DM_PROFILE_PAIRS = 4096;
@@ -376,6 +380,7 @@ extern "C" int dm_destroy(dm_handle* h) {
     cudaFree(h->d_efmt); delete h->h_fmt;
     cudaFree(h->d_pf); cudaFree(h->d_pfmt); cudaFree(h->d_psize); cudaFree(h->d_pout); cudaFreeHost(h->h_pout);
     cudaFreeHost(h->h_ptotal);
+    cudaFree(h->known_buf); cudaFreeHost(h->h_known_hist);
     for (int k = 0; k < 2; ++k) {
         cudaFree(h->d_win[k]);
         if (h->ev_win_done[k]) cudaEventDestroy(h->ev_win_done[k]);
@@ -1384,20 +1389,55 @@ extern "C" int dm_get_global_stats(dm_handle* h, dm_stats_t* out) {
 // ---------------------------------------------------------------------------------------
 // known-set export / import / reset
 // ---------------------------------------------------------------------------------------
+// Every key of the table (own records, peers, dm_import_known), sorted on the device (dm_kernels_window.cuh): the
+// count comes from the table's counter, so a count query (cap 0) copies 8 bytes back and launches nothing.
 extern "C" int dm_export_known(dm_handle* h, uint64_t* keys_out, uint64_t cap, uint64_t* n_out) {
     if (!h || !n_out) return dm_fail(DM_ERR_ARG, "NULL argument");
     DM_CUDA(cudaSetDevice(h->device));
-    DM_CUDA(cudaStreamSynchronize(h->last_stream));
-    // every key of the table (own records, peers, dm_import_known): the slots themselves are read back
-    const uint64_t slots = (uint64_t)h->table.mask + 1;
-    std::vector<unsigned long long> tmp(slots);
-    DM_CUDA(cudaMemcpy(tmp.data(), h->table.slots, slots * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    uint64_t n = 0;
-    for (uint64_t i = 0; i < slots; ++i)
-        if (tmp[i]) tmp[n++] = tmp[i];
-    std::sort(tmp.begin(), tmp.begin() + n);
+    cudaStream_t st = h->last_stream;                    // behind everything the handle enqueued
+    dm_break_chain(h, st);
+    unsigned long long n = 0;
+    DM_CUDA(cudaMemcpyAsync(&n, h->table.count, sizeof(n), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
     *n_out = n;
-    if (keys_out && cap) memcpy(keys_out, tmp.data(), std::min<uint64_t>(n, cap) * sizeof(uint64_t));
+    if (!keys_out || cap == 0 || n == 0) return DM_OK;
+    // the scratch holds the load limit's slots/2 keys; only a table filled past its limit (its training reported
+    // DM_ERR_TABLE_FULL) holds more, and then the scratch grows once to its count
+    const uint64_t slots = (uint64_t)h->table.mask + 1;
+    if (h->known.kcap < n) {
+        cudaFree(h->known_buf);
+        cudaFreeHost(h->h_known_hist);
+        h->known_buf = nullptr;
+        h->h_known_hist = nullptr;
+        h->known.kcap = 0;
+        const uint64_t kcap = std::max<uint64_t>(n, slots / 2);
+        DM_CUDA(cudaMalloc(&h->known_buf, dm_known_scratch(nullptr, kcap, nullptr)));
+        DM_CUDA(cudaHostAlloc(&h->h_known_hist, DMK_HIST_WORDS * sizeof(unsigned int), cudaHostAllocDefault));
+        dm_known_scratch(h->known_buf, kcap, &h->known);
+    }
+    DmKnownScratch& s = h->known;
+    DM_CUDA(cudaMemsetAsync(s.hist, 0, DMK_HIST_WORDS * sizeof(unsigned int), st));
+    dm_k_known_compact<<<dm_grid(slots, DMK_TILE, 4 * (uint64_t)h->sm_count), DMK_THREADS, 0, st>>>(
+        h->table.slots, slots, s.a, s.kcap, s.hist + DMK_PASSES * DMK_BINS);
+    dm_k_known_digits<<<dm_grid(n, DMK_THREADS * 16, 2 * (uint64_t)h->sm_count), DMK_THREADS, 0, st>>>(s.a, n, s.hist);
+    DM_CUDA(cudaGetLastError());
+    DM_CUDA(cudaMemcpyAsync(h->h_known_hist, s.hist, DMK_HIST_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
+    if (h->h_known_hist[DMK_PASSES * DMK_BINS] != n)
+        return dm_fail(DM_ERR_STATE, "the table holds %u keys, its count says %llu", h->h_known_hist[DMK_PASSES * DMK_BINS], n);
+    uint32_t shifts[DMK_PASSES];
+    const uint32_t n_passes = dm_known_passes(h->h_known_hist, n, shifts);
+    const uint32_t tiles = (uint32_t)dm_known_tiles(n);
+    unsigned long long *src = s.a, *dst = s.b;
+    for (uint32_t p = 0; p < n_passes; ++p) {
+        dm_k_known_count<<<tiles, DMK_THREADS, 0, st>>>(src, n, shifts[p], s.counts);
+        dm_alert_scan<uint32_t>(s.counts, (uint64_t)DMK_BINS * tiles, s.tile_sums, s.hist + DMK_PASSES * DMK_BINS + 1, st);
+        dm_k_known_scatter<<<tiles, DMK_THREADS, 0, st>>>(src, n, shifts[p], s.counts, dst);
+        std::swap(src, dst);
+    }
+    DM_CUDA(cudaGetLastError());
+    DM_CUDA(cudaMemcpyAsync(keys_out, src, std::min<uint64_t>(n, cap) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaStreamSynchronize(st));
     return DM_OK;
 }
 

@@ -184,6 +184,12 @@ def b200_detector_service():
 
         _pending_config = None
 
+        def stop(self) -> str:
+            # the engine loop has ended: with params.state_path, what the detector has learnt goes to its state file
+            out = super().stop()
+            self.detector._save_logged("stop()")
+            return out
+
         def reconfigure(self, config_data, persist: bool = False) -> str:
             # the reference validates + stores the new configuration (core.py:299-345); the detector takes it over
             # before the next message

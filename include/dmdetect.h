@@ -351,7 +351,10 @@ int dm_get_anomalies(dm_handle* h, dm_anomaly_t* out, uint32_t cap, uint32_t* n_
 
 int dm_get_stats(dm_handle* h, dm_stats_t* out);
 
-/* Known-set persistence (the reference loses learned state on restart, SURVEY.md 5). */
+/* Known-set persistence (the reference loses learned state on restart, SURVEY.md 5).
+ * dm_export_known: every key of the table, strictly ascending; *n_out = their count, at most cap copied to keys_out
+ * (host memory).  Compaction and sort run on the device; cap 0 (or keys_out NULL) only reads the count.  The first
+ * export that copies keys allocates a device scratch of two slots/2-key buffers, kept until dm_destroy. */
 int dm_export_known(dm_handle* h, uint64_t* keys_out, uint64_t cap, uint64_t* n_out);
 int dm_import_known(dm_handle* h, const uint64_t* keys, uint64_t n);
 /* Forget everything learned and zero the statistics. */
