@@ -396,18 +396,13 @@ class B200NewValueDetector(CoreComponent):
                                                        record_bytes=len(data))
         if train or not flags[0]:
             return None
-        mask = int(masks[0])
-        by_field = dict(vals)
-        alerts = {self.monitors[i].alert_key: _alerts.alert_text(by_field[i])
-                  for i in range(len(self.monitors)) if mask >> i & 1}
-        t = (rec.get("logFormatVariables") or {}).get("Time")
-        return self._detector_schema(rec.get("logID", ""), float(scores[0]), alerts, t)
+        return self._detector_schema(*self._record_alert(rec, vals, int(masks[0]), float(scores[0])))
 
-    def _record_alerts(self, rec: Dict, mask: int) -> Dict[str, str]:
-        """alertsObtain of one anomalous record from the device's unknown-field mask."""
-        by_field = dict(self._record_values(rec))
-        return {self.monitors[i].alert_key: _alerts.alert_text(by_field.get(i, b""))
-                for i in range(len(self.monitors)) if mask >> i & 1}
+    def _record_alert(self, rec: Dict, vals: List[Tuple[int, bytes]], mask: int, score: float) -> tuple:
+        """(logID, score, alertsObtain, Time) of one anomalous ParserSchema record, vals its _record_values."""
+        by_field = dict(vals)
+        return (rec.get("logID", ""), score, self._alerts_of(mask, lambda i: by_field.get(i, b"")),
+                (rec.get("logFormatVariables") or {}).get("Time"))
 
     def _bad_records(self) -> int:
         """The device's count of malformed records (0 for a device stand-in that keeps no statistics)."""
@@ -420,34 +415,24 @@ class B200NewValueDetector(CoreComponent):
         anomalous records to word their alerts."""
         remaining = max(0, self.data_use_training - self.n_seen)
         bad0 = self._bad_records()
-        try:
-            flags, scores, masks = self.det.process_records(data, n_train_records=remaining)
-        except Exception as e:
-            self._count_dropped_training(e, remaining, lambda: len(wire.split_delimited(data)))
-            raise
+        flags, scores, masks = self._device_call(remaining, lambda: len(wire.split_delimited(data)),
+                                                 self.det.process_records, data, n_train_records=remaining)
         n = int(flags.size)
         # malformed records take no training slot (as on the per-record path, where they raise before counting)
         self.last_n_malformed = self._bad_records() - bad0
         self.n_seen += n - self.last_n_malformed
-        if self.output_format == "compact":
-            return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
-        if self.det.last_n_anomalies == 0:
-            return None
-        if self.det.last_n_anomalies >= self.DEVICE_ALERTS_MIN:
-            enc = self._device_alerts(0, n)
-            if enc is not None:
-                return self._device_reply(enc, bare=False)
+        return self._reply(n, flags, scores, self.det.last_n_anomalies, False, 0,
+                           self._record_batch_records, data, flags, scores, masks)
+
+    def _record_batch_records(self, data: bytes, flags, scores, masks):
+        """(logID, score, alertsObtain, Time) of the anomalous records of a ParserSchema batch."""
         frames = wire.split_delimited(data)
-        out = []
         for idx in np.flatnonzero(flags):
             try:
                 rec = wire.decode_parser_schema(frames[int(idx)], strict=False)
             except wire.WireError:
                 continue                     # (a frame the device could walk but the host cannot: skipped, not fatal)
-            alerts = self._record_alerts(rec, int(masks[idx]))
-            t = (rec.get("logFormatVariables") or {}).get("Time")
-            out.append(self._detector_schema(rec.get("logID", ""), float(scores[idx]), alerts, t))
-        return wire.frame_delimited(out) if out else None
+            yield self._record_alert(rec, self._record_values(rec), int(masks[idx]), float(scores[idx]))
 
     # ------------------------------------------------------------------ LogSchema input (the reader stage's records)
     def _process_logs(self, data: bytes, delimited: bool) -> Optional[bytes]:
@@ -457,39 +442,24 @@ class B200NewValueDetector(CoreComponent):
         if len(data) > self.max_batch_bytes:
             raise ValueError(f"a LogSchema message of {len(data)} bytes exceeds max_batch_bytes={self.max_batch_bytes}")
         remaining = max(0, self.data_use_training - self.n_seen)
-        try:
-            flags, scores, n_bad = self.det.process_logs(data, n_train_records=remaining, delimited=delimited)
-        except Exception as e:
-            self._count_dropped_training(e, remaining, lambda: len(wire.split_delimited(data)) if delimited else 1)
-            raise
+        flags, scores, n_bad = self._device_call(remaining, lambda: len(wire.split_delimited(data)) if delimited else 1,
+                                                 self.det.process_logs, data, n_train_records=remaining,
+                                                 delimited=delimited)
         n = int(flags.size)
         self.last_n_malformed = n_bad
         self.n_seen += n - n_bad                                 # malformed and unusable records take no training slot
         if not delimited and n_bad:
             raise wire.WireError("malformed LogSchema record")
-        if self.output_format == "compact":
-            return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
-        if self.det.last_n_anomalies == 0:
-            return None
-        if self.det.last_n_anomalies >= self.DEVICE_ALERTS_MIN:
-            enc = self._device_alerts(0, n)
-            if enc is not None:
-                return self._device_reply(enc, bare=not delimited)
+        return self._reply(n, flags, scores, self.det.last_n_anomalies, not delimited, 0,
+                           self._log_records, data, delimited, scores)
+
+    def _log_records(self, data: bytes, delimited: bool, scores):
+        """(logID, score, alertsObtain, Time) of the anomalous records of the last LogSchema message."""
         frames = wire.split_delimited(data) if delimited else [data]
-        raw_keys = [m.key for m in self.monitors]
-        out = []
         for idx, mask, _offset in self.det.anomalies():
             rec = wire.decode_log_schema(frames[idx])
-            line = wire.log_schema_line(rec)
-            if self.logformat is not None:
-                _eid, variables, lfv = self.logformat.parse(line) or (-1, [], {})
-                alerts, t = self._format_alerts(variables, lfv, mask), lfv.get("Time")
-            else:
-                alerts, t = self._line_alerts(line, mask, raw_keys), _alerts.record_time(line)
-            out.append(self._detector_schema(rec["logID"], float(scores[idx]), alerts, t))
-        if not out:
-            return None
-        return wire.frame_delimited(out) if delimited else out[0]
+            alerts, t = self._text_alerts(wire.log_schema_line(rec), mask)
+            yield rec["logID"], float(scores[idx]), alerts, t
 
     # ------------------------------------------------------------------ raw mode
     def _process_lines(self, data: bytes) -> Optional[bytes]:
@@ -512,9 +482,7 @@ class B200NewValueDetector(CoreComponent):
             pos = end
         if self.output_format == "compact":
             parts = [decode_compact(o) for o in outs]
-            flags = np.concatenate([p[0] for p in parts])
-            scores = np.concatenate([p[1] for p in parts])
-            return struct.pack("<I", flags.size) + flags.tobytes() + scores.tobytes()
+            return _encode_compact(np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts]))
         merged = b"".join(o for o in outs if o)
         return merged or None
 
@@ -604,26 +572,15 @@ class B200NewValueDetector(CoreComponent):
             flags, scores, pieces = self._detect_pipelined(data, self.n_seen)
             n_anom = int(np.count_nonzero(flags))
         else:
-            try:
-                flags, scores = self.det.process_lines(data, n_train_lines=remaining, copy=False)
-            except Exception as e:
-                self._count_dropped_training(e, remaining, lambda: _alerts.count_records(data))
-                raise
+            flags, scores = self._device_call(remaining, lambda: _alerts.count_records(data),
+                                              self.det.process_lines, data, n_train_lines=remaining, copy=False)
             n_anom = self.det.last_n_anomalies
         n = int(flags.size)
         base = self.n_seen
         self.n_seen += n
-        if self.output_format == "compact":
-            return struct.pack("<I", n) + flags.tobytes() + scores.tobytes()
-        if n_anom == 0:
-            return None
         bare = n == 1 and not force_delimited
-        if pieces is None:
-            if n_anom >= self.DEVICE_ALERTS_MIN:
-                enc = self._device_alerts(base, n)
-                if enc is not None:
-                    return self._device_reply(enc, bare=bare)
-            return self._host_line_reply(data, self.det.anomalies(), base, scores, bare)
+        if pieces is None:                                 # (always so for compact output)
+            return self._reply(n, flags, scores, n_anom, bare, base, self._line_records, data, None, base, scores)
         # a pipelined message: the pieces' varint-delimited alerts in order, the host wording those the device did not
         blobs = []
         for p in pieces:
@@ -631,32 +588,24 @@ class B200NewValueDetector(CoreComponent):
                 blobs.append(p[0])
                 self.n_alerts += p[1]
             else:
-                blobs.append(self._host_line_reply(data, p, base, scores, False) or b"")
-        blob = b"".join(blobs)
-        if not blob:
-            return None
-        if bare:
-            _ln, pos = wire._read_varint(blob, 0)
-            return blob[pos:]
-        return blob
+                blobs.append(self._host_alerts(self._line_records(data, p, base, scores)))
+        return _reply_of(b"".join(blobs), bare)
 
-    def _host_line_reply(self, data, anomalies, base: int, scores, bare: bool) -> Optional[bytes]:
-        """The host encoder's reply for raw-line anomalies (record index, mask, byte offset in data)."""
-        out = []
-        raw_keys = [m.key for m in self.monitors]
-        for line_idx, mask, offset in anomalies:
-            rec = _alerts.record_at(data, offset)
-            if self.logformat is not None:
-                _eid, variables, lfv = self.logformat.parse(rec) or (-1, [], {})
-                alerts = self._format_alerts(variables, lfv, mask)
-                out.append(self._detector_schema(str(base + line_idx), float(scores[line_idx]), alerts, lfv.get("Time")))
-                continue
-            alerts = self._line_alerts(rec, mask, raw_keys)
-            out.append(self._detector_schema(str(base + line_idx), float(scores[line_idx]), alerts,
-                                             _alerts.record_time(rec)))
-        if not out:
-            return None
-        return out[0] if bare else wire.frame_delimited(out)
+    def _line_records(self, data, anomalies, base: int, scores):
+        """(logID, score, alertsObtain, Time) of raw-line anomalies (record index, mask, byte offset in data), those of
+        the last batch when anomalies is None; base: the number of the message's first record."""
+        for line_idx, mask, offset in self.det.anomalies() if anomalies is None else anomalies:
+            alerts, t = self._text_alerts(_alerts.record_at(data, offset), mask)
+            yield str(base + line_idx), float(scores[line_idx]), alerts, t
+
+    def _device_call(self, remaining: int, count, call, *args, **kwargs):
+        """call(*args, **kwargs), the device call of a message that trains on up to `remaining` records; should it fail,
+        count() is the message's record count for _count_dropped_training."""
+        try:
+            return call(*args, **kwargs)
+        except Exception as e:
+            self._count_dropped_training(e, remaining, count)
+            raise
 
     def _count_dropped_training(self, err: Exception, remaining: int, count) -> None:
         """A training message the device refused because the known-set table is full (DM_ERR_TABLE_FULL) is dropped by
@@ -670,27 +619,57 @@ class B200NewValueDetector(CoreComponent):
             except Exception:
                 self.n_seen += remaining
 
+    # ------------------------------------------------------------------ alert wording
     @staticmethod
     def _format_value(m: Monitor, variables: List[bytes], lfv: Dict[str, bytes]) -> bytes:
         """Value of monitor m in a record LogFormat.parse split (variables are slices of the normalised Content)."""
         return lfv.get(m.pos, b"") if m.source == "header" else (variables[m.pos] if m.pos < len(variables) else b"")
 
-    def _format_alerts(self, variables: List[bytes], lfv: Dict[str, bytes], mask: int) -> Dict[str, str]:
-        """alertsObtain of one anomalous record in log_format mode from the device's unknown-field mask."""
-        return {m.alert_key: _alerts.alert_text(self._format_value(m, variables, lfv))
-                for i, m in enumerate(self.monitors) if mask >> i & 1}
+    def _text_alerts(self, line: bytes, mask: int) -> Tuple[Dict[str, str], Any]:
+        """alertsObtain and Time value of one anomalous log text (a raw line, or a LogSchema record's `log`): values and
+        Time from the log_format's split, else from the key=value fields (R-tok)."""
+        if self.logformat is not None:
+            _eid, variables, lfv = self.logformat.parse(line) or (-1, [], {})
+            return self._alerts_of(mask, lambda i: self._format_value(self.monitors[i], variables, lfv)), lfv.get("Time")
+        fields = _alerts.record_fields(line, self._quoted_keys(mask))
+        return self._alerts_of(mask, lambda i: fields.get(self.monitors[i].key, b"")), _alerts.record_time(line)
 
-    def _line_alerts(self, rec: bytes, mask: int, raw_keys: List[bytes]) -> Dict[str, str]:
-        """alertsObtain of one anomalous raw record from the device's unknown-field mask."""
-        wanted = [raw_keys[i] for i in range(len(raw_keys)) if mask >> i & 1]
-        vals = _alerts.record_fields(rec, wanted)
-        return {self.monitors[i].alert_key: _alerts.alert_text(vals.get(raw_keys[i], b""))
-                for i in range(len(raw_keys)) if mask >> i & 1}
+    def _quoted_keys(self, mask: int) -> List[bytes]:
+        """The keys of the monitors whose values _alerts_of quotes for an unknown-field mask."""
+        return [m.key for i, m in enumerate(self.monitors) if mask >> i & 1]
+
+    def _alerts_of(self, mask: int, value_of) -> Dict[str, str]:
+        """alertsObtain of one anomalous record: one entry per monitor flagged in the device's unknown-field mask, with
+        value_of(i) the value of monitor i in the record (b"" when it has none).  Of two flagged monitors that share an
+        alert key the last one in config order wins."""
+        return {m.alert_key: _alerts.alert_text(value_of(i)) for i, m in enumerate(self.monitors) if mask >> i & 1}
 
     # ------------------------------------------------------------------ output
+    def _reply(self, n: int, flags, scores, n_anomalies: int, bare: bool, first_log_id: int, host_records, *args):
+        """The reply to a batch of n records: compact output, or None without anomalous records, or their alerts.  From
+        DEVICE_ALERTS_MIN anomalous records on the device encodes the alerts; below that, or when the device declines, the
+        host encodes host_records(*args), which yields (logID, score, alertsObtain, Time) per anomalous record in reply
+        order.  bare: reply with the one DetectorSchema without its length prefix (one record came in).  first_log_id:
+        the number of the batch's first record (raw lines; the record inputs carry their logIDs and pass 0)."""
+        if self.output_format == "compact":
+            return _encode_compact(flags, scores)
+        if n_anomalies == 0:
+            return None
+        if n_anomalies >= self.DEVICE_ALERTS_MIN:
+            enc = self._device_alerts(first_log_id, n)
+            if enc is not None:
+                self.n_alerts += enc[1]
+                return _reply_of(enc[0], bare)
+        return _reply_of(self._host_alerts(host_records(*args)), bare)
+
+    def _host_alerts(self, records) -> bytes:
+        """The host encoder: one DetectorSchema per (logID, score, alertsObtain, Time), numbered as it is written,
+        varint-delimited."""
+        return wire.frame_delimited([self._detector_schema(*r) for r in records])
+
     def _alert_keys(self) -> List[Tuple[str, List[int]]]:
         """alertsObtain keys in the order the host encoder writes them (sorted), each with the mask bits that supply it
-        in config order (two monitors may share a key: the last one flagged wins, as in _line_alerts)."""
+        in config order (two monitors may share a key: the last one flagged wins, as in _alerts_of)."""
         by_key: Dict[str, List[int]] = {}
         for i, m in enumerate(self.monitors):
             by_key.setdefault(m.alert_key, []).append(i)
@@ -720,18 +699,6 @@ class B200NewValueDetector(CoreComponent):
                                  time_capture=names.index("Time") if "Time" in names else None)
             self._alert_sig = sig
         return det.encode_alerts(first_log_id, first_alert_id, now)
-
-    def _device_reply(self, enc: Tuple[bytes, int], bare: bool) -> Optional[bytes]:
-        """The reply made of _device_alerts' result: None without alerts, the one DetectorSchema without its length
-        prefix when one record came in bare, else the varint-delimited DetectorSchemas."""
-        blob, count = enc
-        self.n_alerts += count
-        if not count:
-            return None
-        if bare:
-            _ln, pos = wire._read_varint(blob, 0)
-            return blob[pos:]
-        return blob
 
     def _description(self) -> str:
         return f"{self.detector_id} detects values not encountered in training as anomalies."
@@ -934,15 +901,14 @@ class B200NewValueComboDetector(B200NewValueDetector):
         key = "%s - (%s)" % (scope, ", ".join(self.monitors[i].label for i in members))
         return key, "Unknown value combination: (%s)" % ", ".join("'%s'" % v.decode("utf-8", "replace") for v in values)
 
-    def _record_alerts(self, rec: Dict, mask: int) -> Dict[str, str]:
-        by_field = dict(self._record_values(rec))
+    def _quoted_keys(self, mask: int) -> List[bytes]:
         n = len(self.monitors)
-        return dict(self._combo_alert(members, [by_field.get(i, b"") for i in members])
-                    for c, members in enumerate(self.combos) if mask >> (n + c) & 1)
+        return [self.monitors[i].key for c, members in enumerate(self.combos) if mask >> (n + c) & 1 for i in members]
 
-    def _format_alerts(self, variables: List[bytes], lfv: Dict[str, bytes], mask: int) -> Dict[str, str]:
+    def _alerts_of(self, mask: int, value_of) -> Dict[str, str]:
+        """One entry per combination flagged in the mask (bit len(monitors) + c), quoting its members' values."""
         n = len(self.monitors)
-        return dict(self._combo_alert(members, [self._format_value(self.monitors[i], variables, lfv) for i in members])
+        return dict(self._combo_alert(members, [value_of(i) for i in members])
                     for c, members in enumerate(self.combos) if mask >> (n + c) & 1)
 
     def _process_record(self, data: bytes) -> Optional[bytes]:
@@ -951,31 +917,23 @@ class B200NewValueComboDetector(B200NewValueDetector):
             raise wire.WireError("malformed ParserSchema record")          # as B200NewValueDetector's per-record path
         if out is None or self.output_format == "compact":
             return out
-        return wire.split_delimited(out)[0]                                 # one record in, one bare alert out
+        return _reply_of(out, bare=True)                                    # one record in, one bare alert out
 
-    def _count_dropped_training(self, err: Exception, remaining: int, count) -> None:
-        """A training message the device refused because the known-set table is full (DM_ERR_TABLE_FULL) is dropped by
-        the engine like any failing message (engine.py:192-194) -- but its records still count as seen, otherwise the
-        training window would never end and every later message would fail the same way (the reference's Python sets
-        are unbounded; a larger params.table_log2_slots is the cure)."""
-        from ._lib import DM_ERR_TABLE_FULL
-        if remaining > 0 and getattr(err, "code", None) == DM_ERR_TABLE_FULL:
-            try:
-                self.n_seen += int(count())
-            except Exception:
-                self.n_seen += remaining
 
-    def _line_alerts(self, rec: bytes, mask: int, raw_keys: List[bytes]) -> Dict[str, str]:
-        """Raw key=value records (one thread per record on the device, dm_kernels_lanes.cuh): a
-        combination of global header variables is the tuple of those fields of the record."""
-        n = len(self.monitors)
-        out = {}
-        for c, members in enumerate(self.combos):
-            if mask >> (n + c) & 1:
-                vals = _alerts.record_fields(rec, [raw_keys[i] for i in members])
-                key, text = self._combo_alert(members, [vals.get(raw_keys[i], b"") for i in members])
-                out[key] = text
-        return out
+def _reply_of(blob: bytes, bare: bool) -> Optional[bytes]:
+    """The alerts reply made of varint-delimited DetectorSchemas: None without any, the one DetectorSchema without its
+    length prefix when one record came in bare, else the blob."""
+    if not blob:
+        return None
+    if bare:
+        _ln, pos = wire._read_varint(blob, 0)
+        return blob[pos:]
+    return blob
+
+
+def _encode_compact(flags: np.ndarray, scores: np.ndarray) -> bytes:
+    """The ``compact`` output format: ``<u32 n><n x u8 flag><n x f32 score>``."""
+    return struct.pack("<I", flags.size) + flags.tobytes() + scores.tobytes()
 
 
 def decode_compact(blob: bytes) -> Tuple[np.ndarray, np.ndarray]:
