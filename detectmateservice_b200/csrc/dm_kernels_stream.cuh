@@ -1416,7 +1416,12 @@ static inline int dmx_launch(DmxScratch* s, const uint8_t* d_buf, uint64_t nbyte
         chained = (hint & 0xFFFFFFFFull) != 0 && (hint >> 32) * 4ull >= (hint & 0xFFFFFFFFull);
     }
     s->last_chained = chained;
-    const unsigned grid = dmx_geometry(a, (uint64_t)s->max_grid);
+    const bool pdl = allow_overlap && n_train_lines == 0 && s->chain_stream == st;
+    // A launch that overlaps its predecessor gets half the CTAs that fit on the GPU at once: the other half of every
+    // SM runs the launches next to it, and a warp has twice the rows to spread its fixed costs over (start-up, the
+    // last half-empty field batch).  A launch on its own keeps the full grid.
+    const uint64_t max_grid = pdl ? ((uint64_t)s->max_grid + 1) / 2 : (uint64_t)s->max_grid;
+    const unsigned grid = dmx_geometry(a, max_grid);
     s->last_grid = grid;
     int launched = 0;
     auto bind = [&]() {
@@ -1434,7 +1439,6 @@ static inline int dmx_launch(DmxScratch* s, const uint8_t* d_buf, uint64_t nbyte
         launched += 3;
     }
     bind();
-    const bool pdl = allow_overlap && n_train_lines == 0 && s->chain_stream == st;
     if (mark) mark(mark_ctx, st, 0);
     dm_launch_pdl_smem(chained ? dm_k_stream<false, true> : dm_k_stream<false, false>, grid, DMX_THREADS, (size_t)s->dyn_smem, st, pdl, a);
     if (mark) mark(mark_ctx, st, 1);
