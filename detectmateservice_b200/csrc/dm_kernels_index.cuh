@@ -251,9 +251,11 @@ static inline DmRowsArgs dm_rows_args(const uint8_t* buf, uint64_t nbytes, uint3
 // ---------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------
+#include "dm_buf.h"
+
 struct DmRowsScratch {
-    uint32_t* d_row_prefix = nullptr;
-    unsigned long long* d_tile_state = nullptr;
+    DmDev<uint32_t> d_row_prefix;
+    DmDev<unsigned long long> d_tile_state;
     uint64_t max_rows = 0, max_tiles = 0;
     uint32_t epoch = 0;
     // K_A reads the message before it waits for its predecessor (programmatic dependent launch); a caller may have
@@ -265,16 +267,9 @@ static inline int dm_rows_scratch_create(DmRowsScratch* s, uint64_t max_batch_by
     (void)sm_count;
     s->max_rows = (max_batch_bytes + DMR_ROW - 1) / DMR_ROW + 1;
     s->max_tiles = (s->max_rows + DMR_TILE_ROWS - 1) / DMR_TILE_ROWS + 1;
-    if (cudaMalloc(&s->d_row_prefix, s->max_rows * sizeof(uint32_t)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMalloc(&s->d_tile_state, s->max_tiles * sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMemset(s->d_tile_state, 0, s->max_tiles * sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
+    if (s->d_row_prefix.alloc(s->max_rows) != cudaSuccess) return DM_ERR_CUDA;
+    if (s->d_tile_state.alloc(s->max_tiles, true) != cudaSuccess) return DM_ERR_CUDA;
     return DM_OK;
-}
-
-static inline void dm_rows_scratch_destroy(DmRowsScratch* s) {
-    cudaFree(s->d_row_prefix);
-    cudaFree(s->d_tile_state);
-    s->d_row_prefix = nullptr; s->d_tile_state = nullptr;
 }
 
 // <<<>>> with the programmatic-stream-serialization attribute (see dm_pdl_wait)

@@ -195,7 +195,7 @@ static inline int dm_lanes_launch(DmRowsScratch* s, uint32_t* d_line_start, cons
                                   const void* d_combos, uint32_t n_keys,
                                   cudaStream_t st, void (*mark)(void*, cudaStream_t, int), void* mark_ctx) {
     if ((nbytes + DMR_ROW - 1) / DMR_ROW > s->max_rows) return DM_ERR_CAPACITY;
-    const DmRowsArgs ra = dm_rows_args(d_buf, nbytes, s->d_row_prefix, s->d_tile_state, &s->epoch, d_line_start, d_flags,
+    const DmRowsArgs ra = dm_rows_args(d_buf, nbytes, s->d_row_prefix.get(), s->d_tile_state.get(), &s->epoch, d_line_start, d_flags,
                                        d_scores, out_cap, d_hdr, d_stats, n_train_lines, max_lines);
     if (ra.n_rows == 0) return 0;
     int launched = 0;

@@ -1304,15 +1304,17 @@ static inline unsigned dmx_geometry(DmxArgs& a, uint64_t max_grid) {
 // ---------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------
+#include "dm_buf.h"
+
 struct DmxScratch {
-    DmxKeyTab* d_keys = nullptr;
-    unsigned short* d_row_cnt[DMX_NPAR] = {};
-    unsigned int* d_cta_cnt[DMX_NPAR] = {};
-    unsigned short* d_bound_cnt = nullptr;
-    dm_anomaly_t* d_alerts[DMX_NPAR] = {};
-    unsigned int* d_alert_count = nullptr;      // NPAR words
-    unsigned long long* d_bound = nullptr;
-    DmxShared* d_shared = nullptr;
+    DmDev<DmxKeyTab> d_keys;
+    DmDev<unsigned short> d_row_cnt[DMX_NPAR];
+    DmDev<unsigned int> d_cta_cnt[DMX_NPAR];
+    DmDev<unsigned short> d_bound_cnt;
+    DmDev<dm_anomaly_t> d_alerts[DMX_NPAR];
+    DmDev<unsigned int> d_alert_count;          // NPAR words
+    DmDev<unsigned long long> d_bound;
+    DmDev<DmxShared> d_shared;
     uint32_t alert_cap = 0;
     uint32_t dyn_smem = 0;                      // rings + key table
     uint64_t max_rows = 0;
@@ -1321,23 +1323,20 @@ struct DmxScratch {
     int max_grid = 0;
     bool overlap = false;                       // programmatic dependent launch between consecutive detect launches
     cudaStream_t chain_stream = nullptr;        // stream of the last launch, if it was a plain detect launch (else NULL)
-    unsigned long long* d_timeline = nullptr;   // DM_STREAM_TIMELINE=1
+    DmDev<unsigned long long> d_timeline;       // DM_STREAM_TIMELINE=1
     unsigned last_grid = 0;
     // which instantiation re-checks candidates: 0 = one by one, 1 = chained, 2 = by what the last finished message looked like
     int recheck_mode = 2;
-    unsigned long long* h_hint = nullptr;       // pinned, device-mapped: (batches with a candidate << 32) | rows of that message
+    DmPinned<unsigned long long, cudaHostAllocMapped> h_hint;   // device-mapped: (batches with a candidate << 32) | rows of that message
     bool last_chained = false;
 };
 
-static inline int dmx_scratch_create(DmxScratch* s, const DmKeys& keys, uint64_t max_batch_bytes, uint32_t alert_cap, int sm_count) {
-    DmxKeyTab* t = new (std::nothrow) DmxKeyTab;
+static inline int dmx_scratch_create(DmxScratch* s, const DmKeys& keys, uint64_t max_batch_bytes, uint32_t alert_cap, int sm_count, cudaStream_t st) {
+    std::unique_ptr<DmxKeyTab> t(new (std::nothrow) DmxKeyTab);
     if (!t) return DM_ERR_CUDA;
-    const bool ok = dmx_keytab_build(keys, t);
+    if (!dmx_keytab_build(keys, t.get())) return DM_ERR_CUDA;
     s->dyn_smem = (uint32_t)(DMX_RING_SMEM + ((DMX_KEYTAB_HOT(t->l1_slots) + 15) & ~(size_t)15));
-    cudaError_t e = ok ? cudaMalloc(&s->d_keys, sizeof(DmxKeyTab)) : cudaErrorUnknown;
-    if (e == cudaSuccess) e = cudaMemcpy(s->d_keys, t, sizeof(DmxKeyTab), cudaMemcpyHostToDevice);
-    delete t;
-    if (e != cudaSuccess) return DM_ERR_CUDA;
+    if (dm_upload(s->d_keys, *t, st) != cudaSuccess) return DM_ERR_CUDA;
     s->max_rows = (max_batch_bytes + DMB_ROW - 1) / DMB_ROW + 64;
     s->alert_cap = alert_cap;
     if (cudaFuncSetAttribute(dm_k_stream<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->dyn_smem) != cudaSuccess) return DM_ERR_CUDA;
@@ -1353,8 +1352,7 @@ static inline int dmx_scratch_create(DmxScratch* s, const DmKeys& keys, uint64_t
         if (m && !strcmp(m, "thread")) s->recheck_mode = 0;
         else if (m && !strcmp(m, "chain")) s->recheck_mode = 1;
         else if (m && strcmp(m, "auto") && *m) return DM_ERR_ARG;
-        if (cudaHostAlloc((void**)&s->h_hint, sizeof(unsigned long long), cudaHostAllocMapped) != cudaSuccess) return DM_ERR_CUDA;
-        *s->h_hint = 0;
+        if (s->h_hint.alloc(1, true) != cudaSuccess) return DM_ERR_CUDA;
     }
     if (per_sm < 1) per_sm = 1;
     const char* cap = getenv("DM_STREAM_CTAS_PER_SM");     // tuning knob
@@ -1363,30 +1361,17 @@ static inline int dmx_scratch_create(DmxScratch* s, const DmKeys& keys, uint64_t
     s->max_grid = sm_count * per_sm;
     if (1024u + 4u * (unsigned)s->max_grid > s->dyn_smem) s->max_grid = (int)((s->dyn_smem - 1024u) / 4u);   // (epilogue: per-CTA prefix in shared memory)
     for (unsigned b = 0; b < DMX_NPAR; ++b) {
-        if (cudaMalloc(&s->d_row_cnt[b], s->max_rows * sizeof(unsigned short)) != cudaSuccess) return DM_ERR_CUDA;
-        if (cudaMalloc(&s->d_cta_cnt[b], (size_t)s->max_grid * sizeof(unsigned int)) != cudaSuccess) return DM_ERR_CUDA;
-        if (cudaMalloc(&s->d_alerts[b], (size_t)alert_cap * sizeof(dm_anomaly_t)) != cudaSuccess) return DM_ERR_CUDA;
+        if (s->d_row_cnt[b].alloc(s->max_rows) != cudaSuccess) return DM_ERR_CUDA;
+        if (s->d_cta_cnt[b].alloc(s->max_grid) != cudaSuccess) return DM_ERR_CUDA;
+        if (s->d_alerts[b].alloc(alert_cap) != cudaSuccess) return DM_ERR_CUDA;
     }
-    if (cudaMalloc(&s->d_bound_cnt, s->max_rows * sizeof(unsigned short)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMalloc(&s->d_alert_count, DMX_NPAR * sizeof(unsigned int)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMemset(s->d_alert_count, 0, DMX_NPAR * sizeof(unsigned int)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMalloc(&s->d_bound, sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMalloc(&s->d_shared, sizeof(DmxShared)) != cudaSuccess) return DM_ERR_CUDA;
-    if (cudaMemset(s->d_shared, 0, sizeof(DmxShared)) != cudaSuccess) return DM_ERR_CUDA;
+    if (s->d_bound_cnt.alloc(s->max_rows) != cudaSuccess) return DM_ERR_CUDA;
+    if (s->d_alert_count.alloc(DMX_NPAR, true) != cudaSuccess) return DM_ERR_CUDA;
+    if (s->d_bound.alloc(1) != cudaSuccess) return DM_ERR_CUDA;
+    if (s->d_shared.alloc(1, true) != cudaSuccess) return DM_ERR_CUDA;
     const char* tl = getenv("DM_STREAM_TIMELINE");
-    if (tl && atoi(tl) == 1) {
-        if (cudaMalloc(&s->d_timeline, ((size_t)s->max_grid * 4 + 8) * sizeof(unsigned long long)) != cudaSuccess) return DM_ERR_CUDA;
-        cudaMemset(s->d_timeline, 0, ((size_t)s->max_grid * 4 + 8) * sizeof(unsigned long long));
-    }
+    if (tl && atoi(tl) == 1 && s->d_timeline.alloc((size_t)s->max_grid * 4 + 8, true) != cudaSuccess) return DM_ERR_CUDA;
     return DM_OK;
-}
-
-static inline void dmx_scratch_destroy(DmxScratch* s) {
-    cudaFree(s->d_keys);
-    for (unsigned b = 0; b < DMX_NPAR; ++b) { cudaFree(s->d_row_cnt[b]); cudaFree(s->d_cta_cnt[b]); cudaFree(s->d_alerts[b]); }
-    cudaFree(s->d_bound_cnt); cudaFree(s->d_alert_count); cudaFree(s->d_bound); cudaFree(s->d_shared); cudaFree(s->d_timeline);
-    if (s->h_hint) cudaFreeHost(s->h_hint);
-    *s = DmxScratch();
 }
 
 // Enqueue the kernels for one message.  Returns the number of kernels launched or < 0.  accumulate_errors: the message's
@@ -1401,18 +1386,18 @@ static inline int dmx_launch(DmxScratch* s, const uint8_t* d_buf, uint64_t nbyte
     if (b_rows > s->max_rows) return DM_ERR_CAPACITY;
     DmxArgs a;
     a.buf = d_buf; a.nbytes = nbytes; a.n_rows = n_rows;
-    a.keys = s->d_keys; a.table = table;
+    a.keys = s->d_keys.get(); a.table = table;
     a.flags = d_flags; a.scores = d_scores; a.out_cap = out_cap; a.anomalies = d_anoms; a.anomaly_cap = anomaly_cap;
     a.hdr = d_hdr; a.stats = d_stats; a.n_train_lines = n_train_lines; a.max_lines = max_lines;
-    a.sh = s->d_shared; a.alert_cap = s->alert_cap; a.bound_ptr = nullptr; a.keep_error = 0; a.timeline = s->d_timeline; a.ring_smem = DMX_RING_SMEM;
-    a.error_acc = accumulate_errors ? &s->d_shared->error : nullptr;
+    a.sh = s->d_shared.get(); a.alert_cap = s->alert_cap; a.bound_ptr = nullptr; a.keep_error = 0; a.timeline = s->d_timeline.get(); a.ring_smem = DMX_RING_SMEM;
+    a.error_acc = accumulate_errors ? &s->d_shared.get()->error : nullptr;
     a.keytab_bytes = s->dyn_smem - (uint32_t)DMX_RING_SMEM;
-    a.hint = s->h_hint;                                      // (unified addressing: the mapped host pointer is the device pointer)
+    a.hint = s->h_hint.get();                                      // (unified addressing: the mapped host pointer is the device pointer)
     // chained re-check when, in the last message whose epilogue has run, at least every fourth row had a batch with a
     // candidate (both instantiations give the same results; this only picks the faster one for the stream at hand)
     bool chained = s->recheck_mode == 1;
     if (s->recheck_mode == 2) {
-        const unsigned long long hint = *((volatile unsigned long long*)s->h_hint);
+        const unsigned long long hint = *((volatile unsigned long long*)s->h_hint.get());
         chained = (hint & 0xFFFFFFFFull) != 0 && (hint >> 32) * 4ull >= (hint & 0xFFFFFFFFull);
     }
     s->last_chained = chained;
@@ -1427,13 +1412,13 @@ static inline int dmx_launch(DmxScratch* s, const uint8_t* d_buf, uint64_t nbyte
     auto bind = [&]() {
         a.seq = ++s->seq;
         const int p = (int)(a.seq % DMX_NPAR);
-        a.row_cnt = s->d_row_cnt[p]; a.cta_cnt = s->d_cta_cnt[p]; a.alerts = s->d_alerts[p]; a.alert_count = s->d_alert_count + p;
+        a.row_cnt = s->d_row_cnt[p].get(); a.cta_cnt = s->d_cta_cnt[p].get(); a.alerts = s->d_alerts[p].get(); a.alert_count = s->d_alert_count.get() + p;
     };
     if (n_train_lines > 0) {
         // where detection starts is only known on the device
-        dm_k_rowcount<<<(unsigned)std::min<uint64_t>((b_rows + 7) / 8, 2048), 256, 0, st>>>(d_buf, nbytes, b_rows, s->d_bound_cnt);
-        dm_k_bound<<<1, 256, 0, st>>>(d_buf, nbytes, b_rows, s->d_bound_cnt, n_train_lines, s->d_bound, d_hdr);
-        a.bound_ptr = s->d_bound; a.keep_error = 1;
+        dm_k_rowcount<<<(unsigned)std::min<uint64_t>((b_rows + 7) / 8, 2048), 256, 0, st>>>(d_buf, nbytes, b_rows, s->d_bound_cnt.get());
+        dm_k_bound<<<1, 256, 0, st>>>(d_buf, nbytes, b_rows, s->d_bound_cnt.get(), n_train_lines, s->d_bound.get(), d_hdr);
+        a.bound_ptr = s->d_bound.get(); a.keep_error = 1;
         bind();
         dm_launch_pdl_smem(chained ? dm_k_stream<true, true> : dm_k_stream<true, false>, grid, DMX_THREADS, (size_t)s->dyn_smem, st, false, a);
         launched += 3;

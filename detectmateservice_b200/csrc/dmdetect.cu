@@ -8,10 +8,12 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <vector>
 
+#include "dm_buf.h"
 #include "dm_device.cuh"
 #include "dm_kernels_index.cuh"
 #include "dm_kernels_stream.cuh"
@@ -62,7 +64,7 @@ extern "C" uint64_t dm_table_key(uint32_t field, const uint8_t* value, uint32_t 
 struct dm_handle {
     int device = 0;
     int sm_count = 0;
-    cudaStream_t stream = nullptr;       // the handle's own stream
+    DmStream stream;                     // the handle's own stream
     cudaStream_t last_stream = nullptr;  // stream of the most recent enqueue
     uint64_t max_batch_bytes = 0, max_lines = 0;
     uint32_t table_log2 = 0;
@@ -70,92 +72,88 @@ struct dm_handle {
     int kernel_variant = 6;              // 6 = stream (default), 5 = lanes (one thread per record; DM_KERNEL=lanes)
 
     DmKeys h_keys;
-    DmKeys* d_keys = nullptr;
-    uint8_t* d_in = nullptr;             // staging for host input
-    uint32_t* d_line_start = nullptr;
-    uint8_t* d_flags = nullptr;
-    float* d_scores = nullptr;
-    DmBatchHeader* d_hdr = nullptr;
-    DmBatchHeader* h_hdr = nullptr;      // pinned
-    unsigned int* h_err = nullptr;       // pinned: the stream kernel's error word (DmxShared::error) as dm_sync last read it
-    dm_anomaly_t* d_anoms = nullptr;
+    DmDev<DmKeys> d_keys;
+    DmDev<uint8_t> d_in;                 // staging for host input
+    DmDev<uint32_t> d_line_start;
+    DmDev<uint8_t> d_flags;
+    DmDev<float> d_scores;
+    DmDev<DmBatchHeader> d_hdr;
+    DmPinned<DmBatchHeader> h_hdr;
+    DmPinned<unsigned int> h_err;        // the stream kernel's error word (DmxShared::error) as dm_sync last read it
+    DmDev<dm_anomaly_t> d_anoms;
     uint32_t anomaly_cap = 0;
-    unsigned long long* d_stats = nullptr;         // DM_STATS_WORDS
+    DmDev<unsigned long long> d_stats;   // 3 * DM_STATS_WORDS: own, exported, global
     unsigned long long* d_stats_exported = nullptr;
     unsigned long long* d_stats_global = nullptr;
-    unsigned long long* h_stats = nullptr;         // pinned
-    DmTable table;
+    DmPinned<unsigned long long> h_stats;
+    DmDev<unsigned long long> table_slots, table_novel, table_count;
+    DmTable table;                       // the kernels' view of the three
     uint64_t novel_exported = 0;         // novel keys already shipped in a window
     uint64_t novel_pending = 0;          // novel keys the last window could not carry (more than DM_WINDOW_KEYS learnt)
     DmRowsScratch rows;                  // row / record index scratch (K_A: lanes and log_format kernels)
     DmxScratch dmx;                      // stream-variant scratch (default kernel)
     uint64_t last_nbytes = 0;
-    uint32_t* d_vals = nullptr;          // record mode: offsets / fields / record_of
-    uint64_t vals_cap = 0;
-    uint32_t* d_masks = nullptr;
-    DmMonitors* d_mons = nullptr;        // record mode on the device
+    DmDev<uint32_t> d_vals;              // record mode: offsets / fields / record_of
+    DmDev<uint32_t> d_masks;
+    DmDev<DmMonitors> d_mons;            // record mode on the device
     bool mons_set = false;
     DmMonitors h_mons;             // host copy (dm_set_monitors + dm_set_combos)
-    DmFormat* d_fmt = nullptr;     // log_format + templates (dm_set_format)
-    uint8_t* d_norm = nullptr;     // R-norm: the message's normalised Content text (dm_set_format_ex with flags)
+    DmDev<DmFormat> d_fmt;         // log_format + templates (dm_set_format)
+    DmDev<uint8_t> d_norm;         // R-norm: the message's normalised Content text (dm_set_format_ex with flags)
     bool fmt_norm = false;         // R-norm runs (dm_format_norm)
     void* nccl_comm[2] = {nullptr, nullptr};   // own NCCL communicators (dm_nccl_init): windows alternate between them
     uint32_t nccl_n = 0, nccl_rank = 0, nccl_world = 1;
-    unsigned long long* d_win[2] = {nullptr, nullptr};   // window exchange buffers of dm_window_allreduce
-    cudaEvent_t ev_win_done[2] = {nullptr, nullptr};
+    DmDev<unsigned long long> d_win[2];  // window exchange buffers of dm_window_allreduce
+    DmEvent ev_win_done[2];
     uint64_t win_seq = 0;
-    cudaEvent_t ev_import = nullptr;     // recorded by every dm_window_import, on whichever stream it ran
-    cudaEvent_t ev_order = nullptr;      // dm_use_stream: the previous stream's work, waited for by the next stream
+    DmEvent ev_import;                   // recorded by every dm_window_import, on whichever stream it ran
+    DmEvent ev_order;                    // dm_use_stream: the previous stream's work, waited for by the next stream
     bool fmt_set = false;
     uint32_t fmt_slots = 1;        // DmFormat.max_slots (dynamic shared memory of the thread-per-record kernel)
     // LogSchema input (dm_process_logs), allocated on first use
-    uint8_t* d_logs_text = nullptr;      // the compacted texts + slack
-    uint64_t logs_text_cap = 0;
-    void* d_logs = nullptr;              // per-record / per-line / per-chunk arrays of DmLogsArgs
+    DmDev<uint8_t> d_logs_text;          // the compacted texts + slack
+    DmDev<uint8_t> d_logs;               // per-record / per-line / per-chunk arrays of DmLogsArgs
     uint64_t logs_cap = 0;               // records they hold
     uint32_t logs_chunks = 0;            // chunks they hold
-    DmLogsHeader* d_lhdr = nullptr;
-    DmLogsHeader* h_lhdr = nullptr;      // pinned
+    DmDev<DmLogsHeader> d_lhdr;
+    DmPinned<DmLogsHeader> h_lhdr;
     // DetectorSchema alerts on the device (dm_set_alert_format / dm_encode_alerts), allocated by dm_set_alert_format
     const uint8_t* last_buf = nullptr;   // the last dm_process_lines batch as its kernels read it, and its scores
     const float* last_scores = nullptr;
     uint32_t last_src = DMA_SRC_NONE;    // where the last batch came from: what dm_encode_alerts can word
     uint32_t last_n_records = 0;         // its records (dm_process_records)
-    DmAlertFmt* d_afmt = nullptr;
-    DmAlertHeader* d_ahdr = nullptr;
-    DmAlertHeader* h_ahdr = nullptr;     // pinned
-    void* d_alert = nullptr;             // rank (max_lines + 1), per anomalous record line / mask / offset / size, tile sums
-    uint8_t* d_aout = nullptr;           // the encoded alerts
-    uint64_t alert_cap = 0;              // bytes of d_aout
+    DmDev<DmAlertFmt> d_afmt;
+    DmDev<DmAlertHeader> d_ahdr;
+    DmPinned<DmAlertHeader> h_ahdr;
+    DmDev<uint8_t> d_alert;              // rank (max_lines + 1), per anomalous record line / mask / offset / size, tile sums
+    DmDev<uint8_t> d_aout;               // the encoded alerts
     uint32_t alert_time_cap = DMA_NONE;  // log_format mode: the header capture named Time
-    DmFormat* h_fmt = nullptr;           // host copy of the last dm_set_format[_ex] format (the encoder's is built from it)
-    DmFormat* d_efmt = nullptr;          // the encoder's format: h_fmt keeping the Time capture too (dm_alert_efmt_build)
+    std::unique_ptr<DmFormat> h_fmt;     // host copy of the last dm_set_format[_ex] format (the encoder's is built from it)
+    DmDev<DmFormat> d_efmt;              // the encoder's format: h_fmt keeping the Time capture too (dm_alert_efmt_build)
     uint32_t efmt_slots = 1;
     // the MatcherParser stage (dm_set_parser_format / dm_parse_logs)
-    DmParseFmt* d_pf = nullptr;
-    DmFormat* d_pfmt = nullptr;          // h_fmt keeping every capture (dm_parse_efmt_build)
+    DmDev<DmParseFmt> d_pf;
+    DmDev<DmFormat> d_pfmt;              // h_fmt keeping every capture (dm_parse_efmt_build)
     uint32_t pfmt_slots = 1;
     bool parse_set = false;              // cleared by dm_set_format[_ex]: the parser's format is built from h_fmt
-    unsigned long long* d_psize = nullptr;   // per record its size, then the scan's tile sums and total
-    uint64_t psize_cap = 0;              // records it holds
-    uint8_t* d_pout = nullptr;           // the ParserSchemas, and their pinned host copy
-    uint8_t* h_pout = nullptr;
-    uint64_t pout_cap = 0;
-    unsigned long long* h_ptotal = nullptr;  // pinned
+    DmDev<unsigned long long> d_psize;   // per record its size, then the scan's tile sums and total
+    DmDev<uint8_t> d_pout;               // the ParserSchemas, and their host copy
+    DmPinned<uint8_t> h_pout;
+    DmPinned<unsigned long long> h_ptotal;
     // pipelined host path: two slots
     struct Slot {
-        uint8_t* d_in = nullptr; uint8_t* d_flags = nullptr; float* d_scores = nullptr;
-        DmBatchHeader* d_hdr = nullptr; DmBatchHeader* h_hdr = nullptr; dm_anomaly_t* d_anoms = nullptr;
-        uint8_t* h_flags = nullptr; float* h_scores = nullptr;
-        cudaEvent_t ev_in = nullptr, ev_comp = nullptr, ev_hdr = nullptr;
-        cudaStream_t st_out = nullptr;
+        DmDev<uint8_t> d_in; DmDev<uint8_t> d_flags; DmDev<float> d_scores;
+        DmDev<DmBatchHeader> d_hdr; DmPinned<DmBatchHeader> h_hdr; DmDev<dm_anomaly_t> d_anoms;
+        DmPinned<uint8_t> h_flags; DmPinned<float> h_scores;
+        DmEvent ev_in, ev_comp, ev_hdr;
+        DmStream st_out;
         bool busy = false;
     } slots[2];
-    cudaStream_t st_in = nullptr;
+    DmStream st_in;
     bool slots_ready = false;
     // measurement support
     bool profile = false;
-    std::vector<cudaEvent_t> ev;         // pairs: ev[2i] start, ev[2i+1] stop
+    std::vector<DmEvent> ev;             // pairs: ev[2i] start, ev[2i+1] stop
     size_t ev_used = 0;
     uint64_t launches = 0;               // kernels launched since dm_create
     // A last batch that dm_collect made (dm_encode_alerts): the slot's, for as long as last_src is DMA_LINES and
@@ -163,9 +161,9 @@ struct dm_handle {
     int last_slot = -1;
     uint64_t slot_nbytes[2] = {0, 0};    // the message each slot was submitted last
     // dm_export_known's scratch (dm_known_scratch), allocated by the first export that finds a key
-    void* known_buf = nullptr;
+    DmDev<uint8_t> known_buf;
     DmKnownScratch known{};
-    unsigned int* h_known_hist = nullptr;   // pinned: the digit histograms and the compacted count
+    DmPinned<unsigned int> h_known_hist;    // the digit histograms and the compacted count
 };
 
 static const size_t DM_PROFILE_PAIRS = 4096;
@@ -174,7 +172,7 @@ static void dm_prof_mark(dm_handle* h, cudaStream_t st, int which) {
     if (!h->profile || h->ev_used / 2 >= DM_PROFILE_PAIRS) return;
     if (which == 0 && (h->ev_used & 1)) return;
     if (which == 1 && !(h->ev_used & 1)) return;
-    cudaEventRecord(h->ev[h->ev_used], st);
+    cudaEventRecord(h->ev[h->ev_used].get(), st);
     h->ev_used++;
 }
 
@@ -194,15 +192,15 @@ static void dm_break_chain(dm_handle* h, cudaStream_t st) {
 // chain.  Calls on one stream record and wait on nothing.
 static int dm_use_stream(dm_handle* h, cudaStream_t st) {
     if (st == h->last_stream) return DM_OK;
-    DM_CUDA(cudaEventRecord(h->ev_order, h->last_stream));
-    DM_CUDA(cudaStreamWaitEvent(st, h->ev_order, 0));
+    DM_CUDA(cudaEventRecord(h->ev_order.get(), h->last_stream));
+    DM_CUDA(cudaStreamWaitEvent(st, h->ev_order.get(), 0));
     h->last_stream = st;
     h->dmx.chain_stream = nullptr;
     return DM_OK;
 }
 
 static int dm_pick_stream(dm_handle* h, void* stream, cudaStream_t* out) {
-    *out = stream ? (cudaStream_t)stream : h->stream;
+    *out = stream ? (cudaStream_t)stream : h->stream.get();
     return dm_use_stream(h, *out);
 }
 
@@ -235,45 +233,40 @@ static int dm_create_fill(dm_handle* h, int device, const cudaDeviceProp& prop, 
     }
     dm_keys_finalize_host(&h->h_keys);
 
-    DM_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    h->last_stream = h->stream;
-    DM_CUDA(cudaMalloc(&h->d_keys, sizeof(DmKeys)));
-    DM_CUDA(cudaMemcpy(h->d_keys, &h->h_keys, sizeof(DmKeys), cudaMemcpyHostToDevice));
-    DM_CUDA(cudaMalloc(&h->d_in, max_batch_bytes + 256));
-    DM_CUDA(cudaMemset(h->d_in, 0, max_batch_bytes + 256));
-    DM_CUDA(cudaMalloc(&h->d_line_start, (h->max_lines + 2) * sizeof(uint32_t)));
-    DM_CUDA(cudaMalloc(&h->d_flags, h->max_lines + 16));
-    DM_CUDA(cudaMalloc(&h->d_scores, (h->max_lines + 4) * sizeof(float)));
-    DM_CUDA(cudaMalloc(&h->d_hdr, sizeof(DmBatchHeader)));
-    DM_CUDA(cudaMemset(h->d_hdr, 0, sizeof(DmBatchHeader)));
-    DM_CUDA(cudaHostAlloc(&h->h_hdr, sizeof(DmBatchHeader), cudaHostAllocDefault));
-    memset(h->h_hdr, 0, sizeof(DmBatchHeader));
-    DM_CUDA(cudaHostAlloc(&h->h_err, sizeof(unsigned int), cudaHostAllocDefault));
-    *h->h_err = 0;
+    DM_CUDA(h->stream.create());
+    h->last_stream = h->stream.get();
+    DM_CUDA(dm_upload(h->d_keys, h->h_keys, h->last_stream));
+    DM_CUDA(h->d_in.alloc(max_batch_bytes + 256, true));
+    DM_CUDA(h->d_line_start.alloc(h->max_lines + 2));
+    DM_CUDA(h->d_flags.alloc(h->max_lines + 16));
+    DM_CUDA(h->d_scores.alloc(h->max_lines + 4));
+    DM_CUDA(h->d_hdr.alloc(1, true));
+    DM_CUDA(h->h_hdr.alloc(1, true));
+    DM_CUDA(h->h_err.alloc(1, true));
     h->anomaly_cap = (uint32_t)std::min<uint64_t>(h->max_lines, 1u << 20);
-    DM_CUDA(cudaMalloc(&h->d_anoms, (uint64_t)h->anomaly_cap * sizeof(dm_anomaly_t)));
-    DM_CUDA(cudaMalloc(&h->d_stats, 3 * DM_STATS_WORDS * sizeof(unsigned long long)));
-    DM_CUDA(cudaMemset(h->d_stats, 0, 3 * DM_STATS_WORDS * sizeof(unsigned long long)));
-    h->d_stats_exported = h->d_stats + DM_STATS_WORDS;
-    h->d_stats_global = h->d_stats + 2 * DM_STATS_WORDS;
-    DM_CUDA(cudaHostAlloc(&h->h_stats, DM_STATS_WORDS * sizeof(unsigned long long), cudaHostAllocDefault));
-    DM_CUDA(cudaEventCreateWithFlags(&h->ev_import, cudaEventDisableTiming));
-    DM_CUDA(cudaEventCreateWithFlags(&h->ev_order, cudaEventDisableTiming));
+    DM_CUDA(h->d_anoms.alloc(h->anomaly_cap));
+    DM_CUDA(h->d_stats.alloc(3 * DM_STATS_WORDS, true));
+    h->d_stats_exported = h->d_stats.get() + DM_STATS_WORDS;
+    h->d_stats_global = h->d_stats.get() + 2 * DM_STATS_WORDS;
+    DM_CUDA(h->h_stats.alloc(DM_STATS_WORDS));
+    DM_CUDA(h->ev_import.create());
+    DM_CUDA(h->ev_order.create());
 
     const uint64_t cap = 1ull << table_log2_slots;
     h->table.mask = (uint32_t)(cap - 1);
     h->table.limit = (uint32_t)(cap / 2);
     h->table.novel_cap = (uint32_t)(cap / 2);
-    DM_CUDA(cudaMalloc(&h->table.slots, cap * sizeof(unsigned long long)));
-    DM_CUDA(cudaMemset(h->table.slots, 0, cap * sizeof(unsigned long long)));
-    DM_CUDA(cudaMalloc(&h->table.novel, (cap / 2) * sizeof(unsigned long long)));
-    DM_CUDA(cudaMalloc(&h->table.count, 2 * sizeof(unsigned long long)));
-    DM_CUDA(cudaMemset(h->table.count, 0, 2 * sizeof(unsigned long long)));
+    DM_CUDA(h->table_slots.alloc(cap, true));
+    DM_CUDA(h->table_novel.alloc(cap / 2));
+    DM_CUDA(h->table_count.alloc(2, true));
+    h->table.slots = h->table_slots.get();
+    h->table.novel = h->table_novel.get();
+    h->table.count = h->table_count.get();
     h->table.novel_count = h->table.count + 1;
 
     int rc = dm_rows_scratch_create(&h->rows, max_batch_bytes, h->sm_count);
     if (rc != DM_OK) { return dm_fail(DM_ERR_CUDA, "row index scratch allocation failed: %s", cudaGetErrorString(cudaGetLastError())); }
-    rc = dmx_scratch_create(&h->dmx, h->h_keys, max_batch_bytes, h->anomaly_cap, h->sm_count);
+    rc = dmx_scratch_create(&h->dmx, h->h_keys, max_batch_bytes, h->anomaly_cap, h->sm_count, h->last_stream);
     if (rc == DM_ERR_ARG) return dm_fail(DM_ERR_ARG, "DM_STREAM_RECHECK=%s: thread, chain or auto", getenv("DM_STREAM_RECHECK"));
     if (rc != DM_OK) { return dm_fail(DM_ERR_CUDA, "stream scratch allocation failed: %s", cudaGetErrorString(cudaGetLastError())); }
     { const char* ov = getenv("DM_OVERLAP"); if (ov) h->dmx.overlap = atoi(ov) != 0; }
@@ -316,10 +309,7 @@ extern "C" int dm_create(int device, uint32_t n_keys, const uint8_t* keys_blob, 
     if (!h) return dm_fail(DM_ERR_ARG, "out of host memory");
     const int rc = dm_create_fill(h, device, prop, n_keys, keys_blob, key_lens, max_batch_bytes, max_lines, table_log2_slots);
     if (rc != DM_OK) {
-        char keep[sizeof(g_err)];
-        memcpy(keep, g_err, sizeof(keep));
-        dm_destroy(h);
-        memcpy(g_err, keep, sizeof(keep));
+        dm_destroy(h);                                       // (sets no error message)
         return rc;
     }
     *out = h;
@@ -338,7 +328,7 @@ extern "C" int dm_profile_enable(dm_handle* h, int on) {
     DM_CUDA(cudaSetDevice(h->device));
     if (on && h->ev.empty()) {
         h->ev.resize(2 * DM_PROFILE_PAIRS);
-        for (auto& e : h->ev) DM_CUDA(cudaEventCreate(&e));
+        for (auto& e : h->ev) DM_CUDA(e.create(cudaEventDefault));
     }
     h->profile = on != 0;
     h->ev_used = 0;
@@ -353,7 +343,7 @@ extern "C" int dm_profile_read(dm_handle* h, double* kernel_ms_sum, uint64_t* n_
     const size_t pairs = h->ev_used / 2;
     for (size_t i = 0; i < pairs; ++i) {
         float ms = 0.f;
-        DM_CUDA(cudaEventElapsedTime(&ms, h->ev[2 * i], h->ev[2 * i + 1]));
+        DM_CUDA(cudaEventElapsedTime(&ms, h->ev[2 * i].get(), h->ev[2 * i + 1].get()));
         sum += ms;
     }
     h->ev_used = 0;
@@ -363,48 +353,20 @@ extern "C" int dm_profile_read(dm_handle* h, double* kernel_ms_sum, uint64_t* n_
     return DM_OK;
 }
 
+// The handle's members free what they own when it is deleted: on its device, after everything it enqueued.
 extern "C" int dm_destroy(dm_handle* h) {
     if (!h) return DM_OK;
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
-    for (auto& e : h->ev) cudaEventDestroy(e);
-    dm_rows_scratch_destroy(&h->rows);
-    dmx_scratch_destroy(&h->dmx);
-    cudaFree(h->d_keys); cudaFree(h->d_in);
-    cudaFree(h->d_line_start); cudaFree(h->d_flags); cudaFree(h->d_scores); cudaFree(h->d_hdr);
-    cudaFreeHost(h->h_hdr); cudaFreeHost(h->h_err); cudaFree(h->d_anoms); cudaFree(h->d_stats); cudaFreeHost(h->h_stats);
-    cudaFree(h->table.slots); cudaFree(h->table.novel); cudaFree(h->table.count);
-    cudaFree(h->d_vals); cudaFree(h->d_masks); cudaFree(h->d_mons); cudaFree(h->d_fmt); cudaFree(h->d_norm);
-    cudaFree(h->d_logs_text); cudaFree(h->d_logs); cudaFree(h->d_lhdr); cudaFreeHost(h->h_lhdr);
-    cudaFree(h->d_afmt); cudaFree(h->d_ahdr); cudaFreeHost(h->h_ahdr); cudaFree(h->d_alert); cudaFree(h->d_aout);
-    cudaFree(h->d_efmt); delete h->h_fmt;
-    cudaFree(h->d_pf); cudaFree(h->d_pfmt); cudaFree(h->d_psize); cudaFree(h->d_pout); cudaFreeHost(h->h_pout);
-    cudaFreeHost(h->h_ptotal);
-    cudaFree(h->known_buf); cudaFreeHost(h->h_known_hist);
-    for (int k = 0; k < 2; ++k) {
-        cudaFree(h->d_win[k]);
-        if (h->ev_win_done[k]) cudaEventDestroy(h->ev_win_done[k]);
-        if (h->nccl_comm[k] && g_nccl_destroy_hook) g_nccl_destroy_hook(h->nccl_comm[k]);
-    }
-    for (auto& sl : h->slots) {
-        cudaFree(sl.d_in); cudaFree(sl.d_flags); cudaFree(sl.d_scores); cudaFree(sl.d_hdr); cudaFree(sl.d_anoms);
-        cudaFreeHost(sl.h_hdr); cudaFreeHost(sl.h_flags); cudaFreeHost(sl.h_scores);
-        if (sl.ev_in) cudaEventDestroy(sl.ev_in);
-        if (sl.ev_comp) cudaEventDestroy(sl.ev_comp);
-        if (sl.ev_hdr) cudaEventDestroy(sl.ev_hdr);
-        if (sl.st_out) cudaStreamDestroy(sl.st_out);
-    }
-    if (h->st_in) cudaStreamDestroy(h->st_in);
-    if (h->ev_import) cudaEventDestroy(h->ev_import);
-    if (h->ev_order) cudaEventDestroy(h->ev_order);
-    if (h->stream) cudaStreamDestroy(h->stream);
+    for (void* comm : h->nccl_comm)
+        if (comm && g_nccl_destroy_hook) g_nccl_destroy_hook(comm);
     delete h;
     return DM_OK;
 }
 
 static int dm_check_device_errors(dm_handle* h) {
-    unsigned int err = h->h_hdr->error;
-    if (h->h_hdr->anomaly_list_count > h->anomaly_cap) err |= DM_DEVERR_ANOMALY_OVERFLOW;
+    unsigned int err = h->h_hdr.get()->error;
+    if (h->h_hdr.get()->anomaly_list_count > h->anomaly_cap) err |= DM_DEVERR_ANOMALY_OVERFLOW;
     if (err & DM_DEVERR_TABLE_FULL)
         return dm_fail(DM_ERR_TABLE_FULL, "known-set table over its load limit (2^%u slots); recreate with a larger table_log2_slots", h->table_log2);
     if (err & DM_DEVERR_NOVEL_OVERFLOW)
@@ -420,14 +382,14 @@ static int dm_check_device_errors(dm_handle* h) {
 // dm_process_lines into the handle's error word as well.  Enqueues on st the copy of that word to h_err and its
 // clearing: after st is synchronised, dm_header_with_errors folds it into h_hdr.
 static int dm_fetch_errors(dm_handle* h, cudaStream_t st) {
-    DM_CUDA(cudaMemcpyAsync(h->h_err, &h->dmx.d_shared->error, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
-    DM_CUDA(cudaMemsetAsync(&h->dmx.d_shared->error, 0, sizeof(unsigned int), st));
+    DM_CUDA(cudaMemcpyAsync(h->h_err.get(), &h->dmx.d_shared.get()->error, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemsetAsync(&h->dmx.d_shared.get()->error, 0, sizeof(unsigned int), st));
     return DM_OK;
 }
 
 static int dm_header_with_errors(dm_handle* h) {
-    h->h_hdr->error |= *h->h_err;
-    *h->h_err = 0;
+    h->h_hdr.get()->error |= *h->h_err.get();
+    *h->h_err.get() = 0;
     return dm_check_device_errors(h);
 }
 
@@ -450,13 +412,13 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
 
     const uint8_t* d_buf = buf;
     if (!buf_on_device) {
-        if (nbytes) DM_CUDA(cudaMemcpyAsync(h->d_in, buf, nbytes, cudaMemcpyHostToDevice, st));
-        DM_CUDA(cudaMemsetAsync(h->d_in + nbytes, 0, 64, st));
-        d_buf = h->d_in;
+        if (nbytes) DM_CUDA(cudaMemcpyAsync(h->d_in.get(), buf, nbytes, cudaMemcpyHostToDevice, st));
+        DM_CUDA(cudaMemsetAsync(h->d_in.get() + nbytes, 0, 64, st));
+        d_buf = h->d_in.get();
     }
     const bool host_out = !out_on_device && (flags_out || scores_out);
-    uint8_t* d_flags = (out_on_device && flags_out) ? flags_out : h->d_flags;
-    float* d_scores = (out_on_device && scores_out) ? scores_out : h->d_scores;
+    uint8_t* d_flags = (out_on_device && flags_out) ? flags_out : h->d_flags.get();
+    float* d_scores = (out_on_device && scores_out) ? scores_out : h->d_scores.get();
     // when only one of the two outputs is a caller device buffer the other stays internal
     const uint64_t cap_flags = (out_on_device && flags_out) ? out_cap_lines : h->max_lines;
     const uint64_t cap_scores = (out_on_device && scores_out) ? out_cap_lines : h->max_lines;
@@ -464,47 +426,47 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
 
     bool stream_kernel = false;
     // (the stream kernel and K_A write the per-batch header themselves)
-    if (nbytes == 0) DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+    if (nbytes == 0) DM_CUDA(cudaMemsetAsync(h->d_hdr.get(), 0, sizeof(DmBatchHeader), st));
     h->last_nbytes = nbytes;
 
     if (h->fmt_set) {
         // log_format / template mode: K_A writes the record index, then one THREAD per record
         if ((nbytes + DMR_ROW - 1) / DMR_ROW > h->rows.max_rows) return dm_fail(DM_ERR_CAPACITY, "message too large for the row index");
-        const DmRowsArgs ra = dm_rows_args(d_buf, nbytes, h->rows.d_row_prefix, h->rows.d_tile_state, &h->rows.epoch, h->d_line_start,
-                                           d_flags, d_scores, out_cap, h->d_hdr, h->d_stats, n_train_lines, h->max_lines);
+        const DmRowsArgs ra = dm_rows_args(d_buf, nbytes, h->rows.d_row_prefix.get(), h->rows.d_tile_state.get(), &h->rows.epoch, h->d_line_start.get(),
+                                           d_flags, d_scores, out_cap, h->d_hdr.get(), h->d_stats.get(), n_train_lines, h->max_lines);
         if (ra.n_rows > 0) {
             dm_launch_pdl(dm_k_rowindex, ra.n_tiles, DMR_A_THREADS, st, h->rows.pdl, ra);
             // combination monitors: the COMBO instantiations re-hash their members from the captures the lanes keep
             const bool combos = h->mons_set && h->h_mons.n_combos > 0;
-            DmDetectArgs a = dm_detect_args(d_buf, nbytes, h->d_line_start, h->d_hdr, h->d_keys, h->table, d_flags, d_scores, out_cap,
-                                            h->d_anoms, h->anomaly_cap, h->d_stats, combos ? (const void*)h->d_mons : nullptr);
+            DmDetectArgs a = dm_detect_args(d_buf, nbytes, h->d_line_start.get(), h->d_hdr.get(), h->d_keys.get(), h->table, d_flags, d_scores, out_cap,
+                                            h->d_anoms.get(), h->anomaly_cap, h->d_stats.get(), combos ? (const void*)h->d_mons.get() : nullptr);
             const unsigned grid = dm_detect_grid(nbytes, h->max_lines, DM_FMTL_THREADS, (uint64_t)h->sm_count * 32);
             const size_t smem = (size_t)2 * h->fmt_slots * DM_FMTL_THREADS * sizeof(uint2);
             const bool norm = h->fmt_norm;
             if (n_train_lines > 0) {
                 a.line_lo = 0; a.line_hi = n_train_lines;
                 dm_launch_pdl_smem(dm_format_lanes_kernel(true, norm, combos), grid, DM_FMTL_THREADS, smem, st, false, a,
-                                   (const DmFormat*)h->d_fmt, h->d_norm);
+                                   (const DmFormat*)h->d_fmt.get(), h->d_norm.get());
             }
             a.line_lo = n_train_lines; a.line_hi = ~0ull;
             dm_prof_mark(h, st, 0);
             dm_launch_pdl_smem(dm_format_lanes_kernel(false, norm, combos), grid, DM_FMTL_THREADS, smem, st, false, a,
-                               (const DmFormat*)h->d_fmt, h->d_norm);
+                               (const DmFormat*)h->d_fmt.get(), h->d_norm.get());
             dm_prof_mark(h, st, 1);
             h->launches += 2 + (n_train_lines > 0 ? 1 : 0);
         }
     } else if (h->kernel_variant == 5 || (h->mons_set && h->h_mons.n_combos > 0)) {
         // one thread per record; the only raw-line kernel that evaluates combination monitors
         const bool combos = h->mons_set && h->h_mons.n_combos > 0;
-        const int rc = dm_lanes_launch(&h->rows, h->d_line_start, d_buf, nbytes, n_train_lines, h->d_keys, h->table, d_flags,
-                                       d_scores, out_cap, h->d_anoms, h->anomaly_cap, h->d_hdr, h->d_stats, h->max_lines,
-                                       h->sm_count, combos ? (const void*)h->d_mons : nullptr, h->n_keys, st, dm_prof_mark_cb, h);
+        const int rc = dm_lanes_launch(&h->rows, h->d_line_start.get(), d_buf, nbytes, n_train_lines, h->d_keys.get(), h->table, d_flags,
+                                       d_scores, out_cap, h->d_anoms.get(), h->anomaly_cap, h->d_hdr.get(), h->d_stats.get(), h->max_lines,
+                                       h->sm_count, combos ? (const void*)h->d_mons.get() : nullptr, h->n_keys, st, dm_prof_mark_cb, h);
         if (rc < 0) return dm_fail(DM_ERR_CUDA, "lanes kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         h->launches += (uint64_t)rc;
     } else {
         stream_kernel = true;
-        const int rc = dmx_launch(&h->dmx, d_buf, nbytes, n_train_lines, h->table, d_flags, d_scores, out_cap, h->d_anoms,
-                                  h->anomaly_cap, h->d_hdr, h->d_stats, h->max_lines, st, h->dmx.overlap, true, dm_prof_mark_cb, h);
+        const int rc = dmx_launch(&h->dmx, d_buf, nbytes, n_train_lines, h->table, d_flags, d_scores, out_cap, h->d_anoms.get(),
+                                  h->anomaly_cap, h->d_hdr.get(), h->d_stats.get(), h->max_lines, st, h->dmx.overlap, true, dm_prof_mark_cb, h);
         if (rc < 0) return dm_fail(DM_ERR_CUDA, "stream kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         h->launches += (uint64_t)rc;
     }
@@ -517,20 +479,20 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
     const bool want_sync = host_out || n_lines_out || n_anomalies_out;
     if (!want_sync) return DM_OK;
 
-    DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_hdr.get(), h->d_hdr.get(), sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
     int rc = dm_fetch_errors(h, st);
     if (rc != DM_OK) return rc;
     DM_CUDA(cudaStreamSynchronize(st));
     rc = dm_header_with_errors(h);
     if (rc != DM_OK) return rc;
-    const uint64_t n_lines = h->h_hdr->n_lines;
+    const uint64_t n_lines = h->h_hdr.get()->n_lines;
     if (n_lines_out) *n_lines_out = n_lines;
-    if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    if (n_anomalies_out) *n_anomalies_out = h->h_hdr.get()->n_anomalies;
     if (host_out) {
         if (n_lines > out_cap_lines)
             return dm_fail(DM_ERR_CAPACITY, "batch holds %llu records, output capacity is %llu", (unsigned long long)n_lines, (unsigned long long)out_cap_lines);
-        if (flags_out && n_lines) DM_CUDA(cudaMemcpyAsync(flags_out, h->d_flags, n_lines, cudaMemcpyDeviceToHost, st));
-        if (scores_out && n_lines) DM_CUDA(cudaMemcpyAsync(scores_out, h->d_scores, n_lines * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (flags_out && n_lines) DM_CUDA(cudaMemcpyAsync(flags_out, h->d_flags.get(), n_lines, cudaMemcpyDeviceToHost, st));
+        if (scores_out && n_lines) DM_CUDA(cudaMemcpyAsync(scores_out, h->d_scores.get(), n_lines * sizeof(float), cudaMemcpyDeviceToHost, st));
         DM_CUDA(cudaStreamSynchronize(st));
     }
     return DM_OK;
@@ -544,11 +506,11 @@ extern "C" int dm_process_lines(dm_handle* h, const uint8_t* buf, uint64_t nbyte
 // non-blocking streams, so a later kernel could add to d_stats before the write-back lands.
 static int dm_records_stats(dm_handle* h, cudaStream_t st, uint64_t n_records, uint64_t trained, uint64_t scored, uint64_t nbytes) {
     unsigned long long cur[6];
-    DM_CUDA(cudaMemcpyAsync(cur, h->d_stats, sizeof(cur), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(cur, h->d_stats.get(), sizeof(cur), cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
     dm_stats_add_records(cur, n_records, trained, scored, nbytes);
-    DM_CUDA(cudaMemcpyAsync(h->d_stats, cur, 3 * sizeof(cur[0]), cudaMemcpyHostToDevice, st));
-    DM_CUDA(cudaMemcpyAsync(h->d_stats + 5, &cur[5], sizeof(cur[5]), cudaMemcpyHostToDevice, st));
+    DM_CUDA(cudaMemcpyAsync(h->d_stats.get(), cur, 3 * sizeof(cur[0]), cudaMemcpyHostToDevice, st));
+    DM_CUDA(cudaMemcpyAsync(h->d_stats.get() + 5, &cur[5], sizeof(cur[5]), cudaMemcpyHostToDevice, st));
     DM_CUDA(cudaStreamSynchronize(st));
     return DM_OK;
 }
@@ -568,56 +530,54 @@ extern "C" int dm_process_values(dm_handle* h, const uint8_t* blob, uint64_t blo
             return dm_fail(DM_ERR_ARG, "value %u: field/record/offset out of range", i);
     }
     DM_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = h->stream;
+    cudaStream_t st = h->stream.get();
     int rc = dm_use_stream(h, st);
     if (rc != DM_OK) return rc;
     dm_break_chain(h, st);
     h->last_src = DMA_SRC_NONE;
-    if (n_values > h->vals_cap) {
-        if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
-        h->vals_cap = std::max<uint64_t>(2ull * n_values, 4096);
-        DM_CUDA(cudaMalloc(&h->d_vals, (3 * h->vals_cap + 1) * sizeof(uint32_t)));
-    }
-    if (!h->d_masks) DM_CUDA(cudaMalloc(&h->d_masks, (h->max_lines + 4) * sizeof(uint32_t)));
-    uint32_t* d_off = h->d_vals;
-    uint32_t* d_fld = d_off + h->vals_cap + 1;
-    uint32_t* d_rec = d_fld + h->vals_cap;
-    DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+    // d_vals holds 3 * vals_cap + 1 words: vals_cap + 1 offsets, vals_cap fields, vals_cap records
+    if (n_values > h->d_vals.cap() / 3) DM_CUDA(h->d_vals.grow(3ull * n_values + 1, 3 * std::max<uint64_t>(2ull * n_values, 4096) + 1));
+    DM_CUDA(h->d_masks.alloc(h->max_lines + 4));
+    const uint64_t vals_cap = h->d_vals.cap() / 3;
+    uint32_t* d_off = h->d_vals.get();
+    uint32_t* d_fld = d_off + vals_cap + 1;
+    uint32_t* d_rec = d_fld + vals_cap;
+    DM_CUDA(cudaMemsetAsync(h->d_hdr.get(), 0, sizeof(DmBatchHeader), st));
     if (n_values) {
-        if (blob_bytes) DM_CUDA(cudaMemcpyAsync(h->d_in, blob, blob_bytes, cudaMemcpyHostToDevice, st));
+        if (blob_bytes) DM_CUDA(cudaMemcpyAsync(h->d_in.get(), blob, blob_bytes, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync(d_off, offsets, (uint64_t)(n_values + 1) * 4, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync(d_fld, fields, (uint64_t)n_values * 4, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync(d_rec, record_of, (uint64_t)n_values * 4, cudaMemcpyHostToDevice, st));
     }
     if (n_records) {
-        DM_CUDA(cudaMemsetAsync(h->d_flags, 0, n_records, st));
-        DM_CUDA(cudaMemsetAsync(h->d_scores, 0, (uint64_t)n_records * 4, st));
-        DM_CUDA(cudaMemsetAsync(h->d_masks, 0, (uint64_t)n_records * 4, st));
+        DM_CUDA(cudaMemsetAsync(h->d_flags.get(), 0, n_records, st));
+        DM_CUDA(cudaMemsetAsync(h->d_scores.get(), 0, (uint64_t)n_records * 4, st));
+        DM_CUDA(cudaMemsetAsync(h->d_masks.get(), 0, (uint64_t)n_records * 4, st));
     }
     if (n_values) {
         DmValuesArgs a;
-        a.blob = h->d_in; a.offsets = d_off; a.fields = d_fld; a.record_of = d_rec; a.n_values = n_values;
-        a.n_records = n_records; a.n_train_records = n_train_records; a.keys = h->d_keys; a.table = h->table;
-        a.flags = h->d_flags; a.scores = h->d_scores; a.masks = h->d_masks; a.hdr = h->d_hdr; a.stats = h->d_stats;
+        a.blob = h->d_in.get(); a.offsets = d_off; a.fields = d_fld; a.record_of = d_rec; a.n_values = n_values;
+        a.n_records = n_records; a.n_train_records = n_train_records; a.keys = h->d_keys.get(); a.table = h->table;
+        a.flags = h->d_flags.get(); a.scores = h->d_scores.get(); a.masks = h->d_masks.get(); a.hdr = h->d_hdr.get(); a.stats = h->d_stats.get();
         const int grid = (int)std::min<uint32_t>((n_values + 255) / 256, (uint32_t)h->sm_count * 8);
         if (n_train_records > 0) { dm_k_values<<<grid, 256, 0, st>>>(a, 0); h->launches++; }
         dm_k_values<<<grid, 256, 0, st>>>(a, 1);
         h->launches++;
         DM_CUDA(cudaGetLastError());
     }
-    DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
-    if (flags_out && n_records) DM_CUDA(cudaMemcpyAsync(flags_out, h->d_flags, n_records, cudaMemcpyDeviceToHost, st));
-    if (scores_out && n_records) DM_CUDA(cudaMemcpyAsync(scores_out, h->d_scores, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
-    if (masks_out && n_records) DM_CUDA(cudaMemcpyAsync(masks_out, h->d_masks, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_hdr.get(), h->d_hdr.get(), sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
+    if (flags_out && n_records) DM_CUDA(cudaMemcpyAsync(flags_out, h->d_flags.get(), n_records, cudaMemcpyDeviceToHost, st));
+    if (scores_out && n_records) DM_CUDA(cudaMemcpyAsync(scores_out, h->d_scores.get(), (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
+    if (masks_out && n_records) DM_CUDA(cudaMemcpyAsync(masks_out, h->d_masks.get(), (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
     // statistics that do not need the device: record and byte counts
     const uint32_t tr = std::min<uint32_t>(n_train_records, n_records);
     rc = dm_records_stats(h, st, n_records, tr, n_records - tr, record_bytes);
     if (rc != DM_OK) return rc;
-    h->h_hdr->n_lines = n_records;
+    h->h_hdr.get()->n_lines = n_records;
     rc = dm_check_device_errors(h);
     if (rc != DM_OK) return rc;
-    if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    if (n_anomalies_out) *n_anomalies_out = h->h_hdr.get()->n_anomalies;
     return DM_OK;
 }
 
@@ -639,9 +599,7 @@ extern "C" int dm_set_monitors(dm_handle* h, uint32_t n_monitors, const dm_monit
         memcpy(&hm.m[i], &monitors[i], sizeof(DmMonitor));
     }
     DM_CUDA(cudaSetDevice(h->device));
-    if (!h->d_mons) DM_CUDA(cudaMalloc(&h->d_mons, sizeof(DmMonitors)));
-    DM_CUDA(cudaStreamSynchronize(h->last_stream));
-    DM_CUDA(cudaMemcpy(h->d_mons, &hm, sizeof(DmMonitors), cudaMemcpyHostToDevice));
+    DM_CUDA(dm_upload(h->d_mons, hm, h->last_stream));
     h->mons_set = true;
     return DM_OK;
 }
@@ -670,8 +628,7 @@ extern "C" int dm_set_combos(dm_handle* h, uint32_t n_combos, const uint32_t* me
     for (uint32_t c = 0; c <= n_combos && n_combos; ++c) hm.combo_off[c] = member_off[c];
     for (uint32_t j = 0; n_combos && j < member_off[n_combos]; ++j) hm.combo_members[j] = (uint8_t)members[j];
     DM_CUDA(cudaSetDevice(h->device));
-    DM_CUDA(cudaStreamSynchronize(h->last_stream));
-    DM_CUDA(cudaMemcpy(h->d_mons, &hm, sizeof(DmMonitors), cudaMemcpyHostToDevice));
+    DM_CUDA(dm_upload(h->d_mons, hm, h->last_stream));
     return DM_OK;
 }
 
@@ -695,32 +652,21 @@ extern "C" int dm_set_format_ex(dm_handle* h, const char* log_format, const char
     }
     if (!h->mons_set) return dm_fail(DM_ERR_STATE, "dm_set_monitors has not been called");
     if (n_templates && !templates) return dm_fail(DM_ERR_ARG, "templates is NULL");
-    DmFormat* f = new (std::nothrow) DmFormat;
+    std::unique_ptr<DmFormat> f(new (std::nothrow) DmFormat);
     if (!f) return dm_fail(DM_ERR_CUDA, "out of host memory");
     std::string err;
-    int rc = DM_OK;
-    if (!dm_format_build(log_format, content_name, n_templates, templates, norm_flags, h->h_mons, f, &err)) {
-        rc = dm_fail(DM_ERR_ARG, "%s", err.c_str());
-    } else {
-        cudaError_t e = cudaSetDevice(h->device);
-        if (e == cudaSuccess && !h->d_fmt) e = cudaMalloc(&h->d_fmt, sizeof(DmFormat));
-        if (e == cudaSuccess && norm_flags && n_templates && !h->d_norm) e = cudaMalloc(&h->d_norm, h->max_batch_bytes + 256);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(h->last_stream);
-        if (e == cudaSuccess) e = cudaMemcpy(h->d_fmt, f, sizeof(DmFormat), cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) rc = dm_fail(DM_ERR_CUDA, "dm_set_format: %s", cudaGetErrorString(e));
-        else {
-            h->fmt_set = true;
-            h->fmt_slots = f->max_slots;
-            delete h->h_fmt;
-            h->h_fmt = f;                                        // (kept: the alert encoder's format is built from it)
-            f = nullptr;
-            h->fmt_norm = dm_format_norm(*h->h_fmt);
-            h->parse_set = false;
-        }
-    }
-    delete f;
-    if (rc == DM_OK) rc = dm_alert_efmt_upload(h);
-    return rc;
+    if (!dm_format_build(log_format, content_name, n_templates, templates, norm_flags, h->h_mons, f.get(), &err))
+        return dm_fail(DM_ERR_ARG, "%s", err.c_str());
+    cudaError_t e = cudaSetDevice(h->device);
+    if (e == cudaSuccess && norm_flags && n_templates) e = h->d_norm.alloc(h->max_batch_bytes + 256);
+    if (e == cudaSuccess) e = dm_upload(h->d_fmt, *f, h->last_stream);
+    if (e != cudaSuccess) return dm_fail(DM_ERR_CUDA, "dm_set_format: %s", cudaGetErrorString(e));
+    h->fmt_set = true;
+    h->fmt_slots = f->max_slots;
+    h->h_fmt = std::move(f);                                     // (kept: the alert encoder's format is built from it)
+    h->fmt_norm = dm_format_norm(*h->h_fmt);
+    h->parse_set = false;
+    return dm_alert_efmt_upload(h);
 }
 
 extern "C" int dm_stream_recheck_chained(dm_handle* h) {
@@ -731,14 +677,14 @@ extern "C" int dm_stream_recheck_chained(dm_handle* h) {
 // diagnostics: per-CTA time stamps of the last stream-kernel launch (DM_STREAM_TIMELINE=1)
 extern "C" int dm_debug_rows_timeline(dm_handle* h, unsigned long long* out, uint64_t cap_words, uint32_t* n_warps_out) {
     if (!h || !n_warps_out) return dm_fail(DM_ERR_ARG, "NULL argument");
-    if (h->dmx.d_timeline) {
+    if (h->dmx.d_timeline.get()) {
         // stream variant: per CTA {smid, t_start, t_rows_done, t_exit}, then 8 epilogue stamps
         *n_warps_out = h->dmx.last_grid;
         if (!out) return DM_OK;
         DM_CUDA(cudaSetDevice(h->device));
         DM_CUDA(cudaStreamSynchronize(h->last_stream));
         const uint64_t words = std::min<uint64_t>(cap_words, 4ull * h->dmx.last_grid + 8);
-        DM_CUDA(cudaMemcpy(out, h->dmx.d_timeline, words * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        DM_CUDA(cudaMemcpy(out, h->dmx.d_timeline.get(), words * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
         return DM_OK;
     }
     return dm_fail(DM_ERR_STATE, "create the handle with DM_STREAM_TIMELINE=1");
@@ -767,37 +713,33 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
     if ((flags_out || scores_out || masks_out) && n_records > out_cap)
         return dm_fail(DM_ERR_CAPACITY, "batch holds %u records, output capacity is %llu", n_records, (unsigned long long)out_cap);
     DM_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = h->stream;
+    cudaStream_t st = h->stream.get();
     int rc = dm_use_stream(h, st);
     if (rc != DM_OK) return rc;
     dm_break_chain(h, st);
     h->last_src = DMA_SRC_NONE;
-    if (2ull * n_records + 2 > 3ull * h->vals_cap + 1) {
-        if (h->d_vals) DM_CUDA(cudaFree(h->d_vals));
-        h->vals_cap = std::max<uint64_t>(2ull * n_records, 4096);
-        DM_CUDA(cudaMalloc(&h->d_vals, (3 * h->vals_cap + 1) * sizeof(uint32_t)));
-    }
-    if (!h->d_masks) DM_CUDA(cudaMalloc(&h->d_masks, (h->max_lines + 4) * sizeof(uint32_t)));
-    uint32_t* d_off = h->d_vals;
-    uint32_t* d_len = h->d_vals + n_records;
-    uint32_t* d_bound = h->d_vals + 2ull * n_records;             // {first scored record, records trained}
+    DM_CUDA(h->d_vals.grow(2ull * n_records + 2, 3 * std::max<uint64_t>(2ull * n_records, 4096) + 1));
+    DM_CUDA(h->d_masks.alloc(h->max_lines + 4));
+    uint32_t* d_off = h->d_vals.get();
+    uint32_t* d_len = d_off + n_records;
+    uint32_t* d_bound = d_off + 2ull * n_records;             // {first scored record, records trained}
     uint32_t bound[2] = {0, 0};
-    DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+    DM_CUDA(cudaMemsetAsync(h->d_hdr.get(), 0, sizeof(DmBatchHeader), st));
     if (n_records) {
         // (every record writes its flag, score and mask in the train or the detect launch, malformed ones included)
-        DM_CUDA(cudaMemcpyAsync(h->d_in, buf, nbytes, cudaMemcpyHostToDevice, st));
+        DM_CUDA(cudaMemcpyAsync(h->d_in.get(), buf, nbytes, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync(d_off, off.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync(d_len, len.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
         DmRecordsArgs a;
-        a.buf = h->d_in; a.rec_off = d_off; a.rec_len = d_len; a.n_records = n_records; a.n_train_records = n_train_records;
-        a.mons = h->d_mons; a.table = h->table; a.flags = h->d_flags; a.scores = h->d_scores; a.masks = h->d_masks;
-        a.hdr = h->d_hdr; a.stats = h->d_stats;
+        a.buf = h->d_in.get(); a.rec_off = d_off; a.rec_len = d_len; a.n_records = n_records; a.n_train_records = n_train_records;
+        a.mons = h->d_mons.get(); a.table = h->table; a.flags = h->d_flags.get(); a.scores = h->d_scores.get(); a.masks = h->d_masks.get();
+        a.hdr = h->d_hdr.get(); a.stats = h->d_stats.get();
         const int grid = (int)std::min<uint32_t>((n_records + 127) / 128, (uint32_t)h->sm_count * 16);
         if (n_train_records > 0) {
             // training takes the first n_train_records WELL-FORMED records: mark them (flags as scratch), find the
             // bound, then insert.  Batches after training skip both extra launches.
             dm_k_records<<<grid, 128, 0, st>>>(a, 2);
-            dm_k_records_bound<<<1, 256, 0, st>>>(h->d_flags, n_records, n_train_records, d_bound);
+            dm_k_records_bound<<<1, 256, 0, st>>>(h->d_flags.get(), n_records, n_train_records, d_bound);
             dm_k_records<<<grid, 128, 0, st>>>(a, 0, d_bound);
             h->launches += 3;
         }
@@ -809,21 +751,21 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
         }
         DM_CUDA(cudaGetLastError());
     }
-    DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
-    if (flags_out && n_records) DM_CUDA(cudaMemcpyAsync(flags_out, h->d_flags, n_records, cudaMemcpyDeviceToHost, st));
-    if (scores_out && n_records) DM_CUDA(cudaMemcpyAsync(scores_out, h->d_scores, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
-    if (masks_out && n_records) DM_CUDA(cudaMemcpyAsync(masks_out, h->d_masks, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_hdr.get(), h->d_hdr.get(), sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
+    if (flags_out && n_records) DM_CUDA(cudaMemcpyAsync(flags_out, h->d_flags.get(), n_records, cudaMemcpyDeviceToHost, st));
+    if (scores_out && n_records) DM_CUDA(cudaMemcpyAsync(scores_out, h->d_scores.get(), (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
+    if (masks_out && n_records) DM_CUDA(cudaMemcpyAsync(masks_out, h->d_masks.get(), (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
     if (n_records && n_train_records > 0) DM_CUDA(cudaMemcpyAsync(bound, d_bound, sizeof(bound), cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
     // train_lines: the records trained; detect_lines: the records from the bound on (malformed ones included)
     const uint64_t first_scored = n_train_records > 0 ? bound[0] : 0;
     rc = dm_records_stats(h, st, n_records, bound[1], n_records - first_scored, nbytes);
     if (rc != DM_OK) return rc;
-    h->h_hdr->n_lines = n_records;
+    h->h_hdr.get()->n_lines = n_records;
     rc = dm_check_device_errors(h);
     if (rc != DM_OK) return rc;
     if (n_records_out) *n_records_out = n_records;
-    if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    if (n_anomalies_out) *n_anomalies_out = h->h_hdr.get()->n_anomalies;
     h->last_src = DMA_RECORDS;
     h->last_n_records = n_records;
     return DM_OK;
@@ -836,18 +778,20 @@ extern "C" int dm_process_records(dm_handle* h, const uint8_t* buf, uint64_t nby
 // per-record arrays (dm_logs_scratch_bytes) grow with the largest batch seen; they hold `chunks` walk chunks, the most
 // any of the handle's walk plans makes.
 static int dm_logs_reserve(dm_handle* h, uint64_t n_records, uint32_t chunks) {
-    if (!h->d_lhdr) {
-        DM_CUDA(cudaMalloc(&h->d_lhdr, sizeof(DmLogsHeader)));
-        DM_CUDA(cudaHostAlloc(&h->h_lhdr, sizeof(DmLogsHeader), cudaHostAllocDefault));
-        h->logs_text_cap = dm_logs_text_bytes(h->max_batch_bytes);
-        DM_CUDA(cudaMalloc(&h->d_logs_text, h->logs_text_cap));
+    if (!h->d_lhdr.get()) {                                          // (kept only when all three were allocated)
+        DmDev<DmLogsHeader> d_lhdr; DmPinned<DmLogsHeader> h_lhdr; DmDev<uint8_t> text;
+        DM_CUDA(d_lhdr.alloc(1));
+        DM_CUDA(h_lhdr.alloc(1));
+        DM_CUDA(text.alloc(dm_logs_text_bytes(h->max_batch_bytes)));
+        h->d_lhdr = std::move(d_lhdr);
+        h->h_lhdr = std::move(h_lhdr);
+        h->d_logs_text = std::move(text);
     }
     if (n_records <= h->logs_cap) return DM_OK;
     const uint64_t cap = std::min<uint64_t>(std::max<uint64_t>({n_records, 2 * h->logs_cap, 4096}), h->max_lines);
-    if (h->d_logs) DM_CUDA(cudaFree(h->d_logs));
-    h->d_logs = nullptr;
+    const uint64_t bytes = dm_logs_scratch_bytes(cap, chunks);
     h->logs_cap = 0;
-    DM_CUDA(cudaMalloc(&h->d_logs, dm_logs_scratch_bytes(cap, chunks)));
+    DM_CUDA(h->d_logs.grow(bytes, bytes));
     h->logs_cap = cap;
     h->logs_chunks = chunks;
     return DM_OK;
@@ -870,7 +814,7 @@ static int dm_logs_unwrap(dm_handle* h, const uint8_t* buf, uint64_t nbytes, con
                           bool copy, DmLogsArgs* out, float** d_rscores, uint8_t** d_rflags) {
     const uint32_t n_records = (uint32_t)fr.off.size();
     DM_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = h->stream;
+    cudaStream_t st = h->stream.get();
     int rc = dm_use_stream(h, st);
     if (rc != DM_OK) return rc;
     dm_break_chain(h, st);
@@ -878,10 +822,10 @@ static int dm_logs_unwrap(dm_handle* h, const uint8_t* buf, uint64_t nbytes, con
     const uint32_t walk_ctas = (uint32_t)h->sm_count * 4;
     rc = dm_logs_reserve(h, n_records, walk_ctas);
     if (rc != DM_OK) return rc;
-    DmLogsArgs a = dm_logs_carve(h->d_logs, h->logs_cap, h->logs_chunks, h->d_lhdr, d_rscores, d_rflags);
-    dm_logs_call(&a, h->d_in, n_records, n_train_records, walk_ctas, copy ? h->d_logs_text : nullptr,
-                 copy ? h->logs_text_cap : 0);
-    if (nbytes) DM_CUDA(cudaMemcpyAsync(h->d_in, buf, nbytes, cudaMemcpyHostToDevice, st));
+    DmLogsArgs a = dm_logs_carve(h->d_logs.get(), h->logs_cap, h->logs_chunks, h->d_lhdr.get(), d_rscores, d_rflags);
+    dm_logs_call(&a, h->d_in.get(), n_records, n_train_records, walk_ctas, copy ? h->d_logs_text.get() : nullptr,
+                 copy ? h->d_logs_text.cap() : 0);
+    if (nbytes) DM_CUDA(cudaMemcpyAsync(h->d_in.get(), buf, nbytes, cudaMemcpyHostToDevice, st));
     if (n_records) {
         DM_CUDA(cudaMemcpyAsync((void*)a.rec_off, fr.off.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
         DM_CUDA(cudaMemcpyAsync((void*)a.rec_len, fr.len.data(), (uint64_t)n_records * 4, cudaMemcpyHostToDevice, st));
@@ -895,9 +839,9 @@ static int dm_logs_unwrap(dm_handle* h, const uint8_t* buf, uint64_t nbytes, con
         }
         DM_CUDA(cudaGetLastError());
     } else {
-        DM_CUDA(cudaMemsetAsync(h->d_lhdr, 0, sizeof(DmLogsHeader), st));
+        DM_CUDA(cudaMemsetAsync(h->d_lhdr.get(), 0, sizeof(DmLogsHeader), st));
     }
-    DM_CUDA(cudaMemcpyAsync(h->h_lhdr, h->d_lhdr, sizeof(DmLogsHeader), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_lhdr.get(), h->d_lhdr.get(), sizeof(DmLogsHeader), cudaMemcpyDeviceToHost, st));
     *out = a;
     return DM_OK;
 }
@@ -919,33 +863,33 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
     uint8_t* d_rflags;
     rc = dm_logs_unwrap(h, buf, nbytes, fr, n_train_records, true, &a, &d_rscores, &d_rflags);
     if (rc != DM_OK) return rc;
-    cudaStream_t st = h->stream;
+    cudaStream_t st = h->stream.get();
     DM_CUDA(cudaStreamSynchronize(st));
-    const DmLogsHeader lh = *h->h_lhdr;
+    const DmLogsHeader lh = *h->h_lhdr.get();
     if (lh.n_lines) {
         uint64_t n_lines = 0, n_anoms = 0;
-        rc = dm_process_lines(h, h->d_logs_text, lh.total_bytes, 1, lh.n_train, nullptr, nullptr, 0, 0, &n_lines, &n_anoms, st);
+        rc = dm_process_lines(h, h->d_logs_text.get(), lh.total_bytes, 1, lh.n_train, nullptr, nullptr, 0, 0, &n_lines, &n_anoms, st);
         dm_break_chain(h, st);
         h->last_src = DMA_SRC_NONE;                           // (its anomaly list is rewritten to records below)
         if (rc != DM_OK) return rc;
         if (n_lines != lh.n_lines)
             return dm_fail(DM_ERR_STATE, "the line path found %llu records in %llu unwrapped texts", (unsigned long long)n_lines, (unsigned long long)lh.n_lines);
     } else {
-        DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+        DM_CUDA(cudaMemsetAsync(h->d_hdr.get(), 0, sizeof(DmBatchHeader), st));
         h->last_src = DMA_SRC_NONE;
     }
     const unsigned grid_s = dm_logs_scatter_grid(n_records, h->anomaly_cap, (uint64_t)h->sm_count * 8);
-    dm_k_logs_scatter<<<grid_s, DML_THREADS, 0, st>>>(a, h->d_flags, h->d_scores, d_rflags, d_rscores, h->d_anoms, h->anomaly_cap,
-                                                     h->d_hdr, h->d_stats, nbytes);
+    dm_k_logs_scatter<<<grid_s, DML_THREADS, 0, st>>>(a, h->d_flags.get(), h->d_scores.get(), d_rflags, d_rscores, h->d_anoms.get(), h->anomaly_cap,
+                                                     h->d_hdr.get(), h->d_stats.get(), nbytes);
     h->launches++;
     DM_CUDA(cudaGetLastError());
-    DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_hdr.get(), h->d_hdr.get(), sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, st));
     if (flags_out && n_records) DM_CUDA(cudaMemcpyAsync(flags_out, d_rflags, n_records, cudaMemcpyDeviceToHost, st));
     if (scores_out && n_records) DM_CUDA(cudaMemcpyAsync(scores_out, d_rscores, (uint64_t)n_records * 4, cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
     if (n_records_out) *n_records_out = n_records;
     if (n_malformed_out) *n_malformed_out = n_records - lh.n_lines;
-    if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    if (n_anomalies_out) *n_anomalies_out = h->h_hdr.get()->n_anomalies;
     h->last_src = DMA_LOGS;                                   // (the line path left last_buf / last_nbytes: the texts)
     h->last_scores = d_rscores;
     return DM_OK;
@@ -957,16 +901,13 @@ extern "C" int dm_process_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes
 // The encoder's copy of the log_format (when both the format and the alert format are set): the matcher's own, keeping
 // the Time capture as well.
 static int dm_alert_efmt_upload(dm_handle* h) {
-    if (!h->fmt_set || !h->h_fmt || !h->d_afmt) return DM_OK;
-    DmFormat* ef = new (std::nothrow) DmFormat;
+    if (!h->fmt_set || !h->h_fmt || !h->d_afmt.get()) return DM_OK;
+    std::unique_ptr<DmFormat> ef(new (std::nothrow) DmFormat);
     if (!ef) return dm_fail(DM_ERR_ARG, "out of host memory");
-    dm_alert_efmt_build(*h->h_fmt, h->alert_time_cap, ef);
+    dm_alert_efmt_build(*h->h_fmt, h->alert_time_cap, ef.get());
     cudaError_t e = cudaSetDevice(h->device);
-    if (e == cudaSuccess && !h->d_efmt) e = cudaMalloc(&h->d_efmt, sizeof(DmFormat));
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->last_stream);
-    if (e == cudaSuccess) e = cudaMemcpy(h->d_efmt, ef, sizeof(DmFormat), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = dm_upload(h->d_efmt, *ef, h->last_stream);
     if (e == cudaSuccess) h->efmt_slots = ef->max_slots;
-    delete ef;
     if (e != cudaSuccess) return dm_fail(DM_ERR_CUDA, "encoder format: %s", cudaGetErrorString(e));
     return DM_OK;
 }
@@ -978,39 +919,34 @@ extern "C" int dm_set_alert_format(dm_handle* h, uint32_t n_strings, const uint8
     if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
     if (!string_lens || (!strings && n_strings)) return dm_fail(DM_ERR_ARG, "strings missing");
     if (out_cap == 0) return dm_fail(DM_ERR_ARG, "out_cap must be positive");
-    DmAlertFmt* f = new (std::nothrow) DmAlertFmt;
+    std::unique_ptr<DmAlertFmt> f(new (std::nothrow) DmAlertFmt);
     if (!f) return dm_fail(DM_ERR_ARG, "out of host memory");
     const char* why = dm_alert_fmt_build(h->h_keys, n_strings, strings, string_lens, bits_off, bits, n_combos, combo_off,
-                                         combo_members, time_capture, f);
-    if (why) { delete f; return dm_fail(DM_ERR_ARG, "dm_set_alert_format: %s", why); }
+                                         combo_members, time_capture, f.get());
+    if (why) return dm_fail(DM_ERR_ARG, "dm_set_alert_format: %s", why);
     cudaError_t e = cudaSetDevice(h->device);
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->last_stream);
-    if (e == cudaSuccess && !h->d_afmt) {
+    if (e == cudaSuccess && !h->d_afmt.get()) {
         // everything the encoder needs, once: per record a rank, per anomaly-list entry a record's line, mask, offset and
-        // size, the scan's tile sums.  Allocated into locals and kept only when every allocation succeeded, so that a
-        // failed call leaves the handle without an encoder (and a later call allocates again).
-        DmAlertFmt* d_afmt = nullptr;
-        DmAlertHeader *d_ahdr = nullptr, *h_ahdr = nullptr;
-        void* d_alert = nullptr;
-        e = cudaMalloc(&d_afmt, sizeof(DmAlertFmt));
-        if (e == cudaSuccess) e = cudaMalloc(&d_ahdr, sizeof(DmAlertHeader));
-        if (e == cudaSuccess) e = cudaHostAlloc(&h_ahdr, sizeof(DmAlertHeader), cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaMalloc(&d_alert, dm_alert_scratch(nullptr, h->max_lines, h->anomaly_cap, nullptr, nullptr));
+        // size, the scan's tile sums.  Kept only when every allocation succeeded, so that a failed call leaves the
+        // handle without an encoder (and a later call allocates again).
+        DmDev<DmAlertFmt> d_afmt;
+        DmDev<DmAlertHeader> d_ahdr;
+        DmPinned<DmAlertHeader> h_ahdr;
+        DmDev<uint8_t> d_alert;
+        e = d_afmt.alloc(1);
+        if (e == cudaSuccess) e = d_ahdr.alloc(1);
+        if (e == cudaSuccess) e = h_ahdr.alloc(1);
+        if (e == cudaSuccess) e = d_alert.alloc(dm_alert_scratch(nullptr, h->max_lines, h->anomaly_cap, nullptr, nullptr));
         if (e == cudaSuccess) {
-            h->d_afmt = d_afmt; h->d_ahdr = d_ahdr; h->h_ahdr = h_ahdr; h->d_alert = d_alert;
-        } else {
-            cudaFree(d_afmt); cudaFree(d_ahdr); cudaFreeHost(h_ahdr); cudaFree(d_alert);
+            h->d_afmt = std::move(d_afmt); h->d_ahdr = std::move(d_ahdr); h->h_ahdr = std::move(h_ahdr); h->d_alert = std::move(d_alert);
         }
     }
-    if (e == cudaSuccess && out_cap != h->alert_cap) {
-        cudaFree(h->d_aout);
-        h->d_aout = nullptr;
-        h->alert_cap = 0;
-        e = cudaMalloc(&h->d_aout, out_cap);
-        if (e == cudaSuccess) h->alert_cap = out_cap;
+    if (e == cudaSuccess && out_cap != h->d_aout.cap()) {
+        h->d_aout.reset();
+        e = h->d_aout.alloc(out_cap);
     }
-    if (e == cudaSuccess) e = cudaMemcpy(h->d_afmt, f, sizeof(DmAlertFmt), cudaMemcpyHostToDevice);
-    delete f;
+    if (e == cudaSuccess) e = dm_upload(h->d_afmt, *f, h->last_stream);
     if (e != cudaSuccess) return dm_fail(DM_ERR_CUDA, "dm_set_alert_format: %s", cudaGetErrorString(e));
     h->alert_time_cap = time_capture < DM_FMT_MAX_CAPTURES ? time_capture : DMA_NONE;
     return dm_alert_efmt_upload(h);
@@ -1028,7 +964,7 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
                                 uint64_t out_cap, uint64_t* out_len, uint64_t* n_alerts, int* declined) {
     if (!h || !out_len || !n_alerts || !declined) return dm_fail(DM_ERR_ARG, "NULL argument");
     if (out_cap && !out) return dm_fail(DM_ERR_ARG, "out is NULL");
-    if (!h->d_afmt || !h->d_aout) return dm_fail(DM_ERR_STATE, "dm_set_alert_format has not been called");
+    if (!h->d_afmt.get() || !h->d_aout.get()) return dm_fail(DM_ERR_STATE, "dm_set_alert_format has not been called");
     if (h->last_src == DMA_SRC_NONE)
         return dm_fail(DM_ERR_STATE, "the last batch did not come from dm_process_lines, dm_process_logs, dm_process_records "
                                      "or dm_collect");
@@ -1038,7 +974,7 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     // A collected slot: its kernels have finished (dm_collect waited for them) and its header is the one dm_collect
     // read; dm_sync would put the handle's own header in its place.  The encoder runs on the slot's output stream, so
     // the other slot's kernels, in flight on the compute stream, keep running and their overlap chain stays intact.
-    const bool from_slot = h->last_src == DMA_LINES && h->last_slot >= 0 && h->last_buf == h->slots[h->last_slot].d_in;
+    const bool from_slot = h->last_src == DMA_LINES && h->last_slot >= 0 && h->last_buf == h->slots[h->last_slot].d_in.get();
     const dm_handle::Slot* sl = from_slot ? &h->slots[h->last_slot] : nullptr;
     if (sl) {
         DM_CUDA(cudaSetDevice(h->device));
@@ -1049,7 +985,7 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     const uint32_t src = h->last_src;
     uint64_t n_lines;
     bool over;
-    const uint64_t n_flagged = dm_alert_entries(src, sl ? *sl->h_hdr : *h->h_hdr, h->last_n_records, h->anomaly_cap, &n_lines,
+    const uint64_t n_flagged = dm_alert_entries(src, sl ? *sl->h_hdr.get() : *h->h_hdr.get(), h->last_n_records, h->anomaly_cap, &n_lines,
                                                 &over);
     if (over) {
         *n_alerts = n_flagged;
@@ -1058,26 +994,26 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     }
     if (n_flagged == 0) return DM_OK;
     const uint32_t entries = (uint32_t)n_flagged;
-    cudaStream_t st = sl ? sl->st_out : h->last_stream;
+    cudaStream_t st = sl ? sl->st_out.get() : h->last_stream;
     dm_break_chain(h, st);
     DmAlertArgs a;
     unsigned long long* tile_sums;
-    dm_alert_scratch((uint8_t*)h->d_alert, h->max_lines, h->anomaly_cap, &a, &tile_sums);
-    a.fmt = h->d_afmt; a.buf = h->last_buf; a.nbytes = h->last_nbytes; a.scores = h->last_scores;
-    a.anoms = sl ? sl->d_anoms : h->d_anoms; a.n_entries = entries; a.n_lines = n_lines;
-    a.ahdr = h->d_ahdr; a.first_log_id = first_log_id; a.first_alert_id = first_alert_id; a.now = now;
-    a.out = h->d_aout; a.out_cap = std::min(out_cap, h->alert_cap);
-    a.efmt = h->d_efmt; a.nbuf = h->d_norm;
+    dm_alert_scratch((uint8_t*)h->d_alert.get(), h->max_lines, h->anomaly_cap, &a, &tile_sums);
+    a.fmt = h->d_afmt.get(); a.buf = h->last_buf; a.nbytes = h->last_nbytes; a.scores = h->last_scores;
+    a.anoms = sl ? sl->d_anoms.get() : h->d_anoms.get(); a.n_entries = entries; a.n_lines = n_lines;
+    a.ahdr = h->d_ahdr.get(); a.first_log_id = first_log_id; a.first_alert_id = first_alert_id; a.now = now;
+    a.out = h->d_aout.get(); a.out_cap = std::min<uint64_t>(out_cap, h->d_aout.cap());
+    a.efmt = h->d_efmt.get(); a.nbuf = h->d_norm.get();
     a.src = src;
     if (src == DMA_LOGS) {
         float* rscores;
         uint8_t* rflags;
-        const DmLogsArgs la = dm_logs_carve(h->d_logs, h->logs_cap, h->logs_chunks, h->d_lhdr, &rscores, &rflags);
-        a.pay = h->d_in; a.pay_off = la.rec_off; a.pay_len = la.rec_len;
+        const DmLogsArgs la = dm_logs_carve(h->d_logs.get(), h->logs_cap, h->logs_chunks, h->d_lhdr.get(), &rscores, &rflags);
+        a.pay = h->d_in.get(); a.pay_off = la.rec_off; a.pay_len = la.rec_len;
         a.log_line = la.rec_line; a.log_dst = la.line_dst;
     } else if (src == DMA_RECORDS) {
-        a.pay = h->d_in; a.pay_off = h->d_vals; a.pay_len = h->d_vals + n_lines;
-        a.scores = h->d_scores; a.flags = h->d_flags; a.masks = h->d_masks; a.mons = h->d_mons;
+        a.pay = h->d_in.get(); a.pay_off = h->d_vals.get(); a.pay_len = h->d_vals.get() + n_lines;
+        a.scores = h->d_scores.get(); a.flags = h->d_flags.get(); a.masks = h->d_masks.get(); a.mons = h->d_mons.get();
     }
     bool fmtl;
     uint64_t mark_n;
@@ -1086,29 +1022,29 @@ extern "C" int dm_encode_alerts(dm_handle* h, uint64_t first_log_id, int64_t fir
     const DmAlertKernel k_size = dm_alert_pass_kernel(src, h->fmt_set, h->fmt_norm, false, &fmtl);
     const DmAlertKernel k_write = dm_alert_pass_kernel(src, h->fmt_set, h->fmt_norm, true, &fmtl);
     // log_format mode: the size and write passes re-run the matcher (one thread per record, DM_FMTL_THREADS per CTA)
-    if (fmtl && !h->d_efmt) return dm_fail(DM_ERR_STATE, "no log_format for the alert encoder");
+    if (fmtl && !h->d_efmt.get()) return dm_fail(DM_ERR_STATE, "no log_format for the alert encoder");
     const unsigned mgrid = dm_grid(mark_n, DMA_THREADS, (uint64_t)h->sm_count * 8);
     const unsigned threads = fmtl ? DM_FMTL_THREADS : DMA_THREADS;
     const unsigned pgrid = dm_grid(entries, threads, (uint64_t)h->sm_count * (fmtl ? 32 : 8));
     const size_t smem = fmtl ? (size_t)2 * h->efmt_slots * DM_FMTL_THREADS * sizeof(uint2) : 0;
-    DM_CUDA(cudaMemsetAsync(h->d_ahdr, 0, sizeof(DmAlertHeader), st));
+    DM_CUDA(cudaMemsetAsync(h->d_ahdr.get(), 0, sizeof(DmAlertHeader), st));
     DM_CUDA(cudaMemsetAsync(a.rank, 0, n_lines * 4, st));
     DM_CUDA(cudaMemsetAsync(a.rec_mask, 0, (uint64_t)entries * 4, st));
     k_mark<<<mgrid, DMA_THREADS, 0, st>>>(a);
-    dm_alert_scan<uint32_t>(a.rank, n_lines, (uint32_t*)tile_sums, &h->d_ahdr->n_alerts, st);
+    dm_alert_scan<uint32_t>(a.rank, n_lines, (uint32_t*)tile_sums, &h->d_ahdr.get()->n_alerts, st);
     k_gather<<<mgrid, DMA_THREADS, 0, st>>>(a);
     k_size<<<pgrid, threads, smem, st>>>(a);
-    dm_alert_scan<unsigned long long>(a.size, entries, tile_sums, &h->d_ahdr->total, st);
+    dm_alert_scan<unsigned long long>(a.size, entries, tile_sums, &h->d_ahdr.get()->total, st);
     k_write<<<pgrid, threads, smem, st>>>(a);
     h->launches += 10;
     DM_CUDA(cudaGetLastError());
-    DM_CUDA(cudaMemcpyAsync(h->h_ahdr, h->d_ahdr, sizeof(DmAlertHeader), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_ahdr.get(), h->d_ahdr.get(), sizeof(DmAlertHeader), cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
-    const DmAlertHeader ah = *h->h_ahdr;
+    const DmAlertHeader ah = *h->h_ahdr.get();
     *n_alerts = ah.n_alerts;
     *out_len = ah.total;
     if (ah.declined || ah.total > a.out_cap) { *declined = 1; return DM_OK; }
-    if (ah.total) DM_CUDA(cudaMemcpyAsync(out, h->d_aout, ah.total, cudaMemcpyDeviceToHost, st));
+    if (ah.total) DM_CUDA(cudaMemcpyAsync(out, h->d_aout.get(), ah.total, cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
     return DM_OK;
 }
@@ -1124,22 +1060,17 @@ extern "C" int dm_set_parser_format(dm_handle* h, uint32_t n_strings, const uint
     if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
     if (!h->fmt_set || !h->h_fmt) return dm_fail(DM_ERR_STATE, "dm_set_format has not been called");
     if (!string_lens || (!strings && n_strings)) return dm_fail(DM_ERR_ARG, "strings missing");
-    DmParseFmt* P = new (std::nothrow) DmParseFmt;
-    DmFormat* pf = new (std::nothrow) DmFormat;
-    if (!P || !pf) { delete P; delete pf; return dm_fail(DM_ERR_ARG, "out of host memory"); }
-    const char* why = dm_parse_fmt_build(*h->h_fmt, n_strings, strings, string_lens, capture_order, P);
-    if (why) { delete P; delete pf; return dm_fail(DM_ERR_ARG, "dm_set_parser_format: %s", why); }
-    dm_parse_efmt_build(*h->h_fmt, pf);
+    std::unique_ptr<DmParseFmt> P(new (std::nothrow) DmParseFmt);
+    std::unique_ptr<DmFormat> pf(new (std::nothrow) DmFormat);
+    if (!P || !pf) return dm_fail(DM_ERR_ARG, "out of host memory");
+    const char* why = dm_parse_fmt_build(*h->h_fmt, n_strings, strings, string_lens, capture_order, P.get());
+    if (why) return dm_fail(DM_ERR_ARG, "dm_set_parser_format: %s", why);
+    dm_parse_efmt_build(*h->h_fmt, pf.get());
     cudaError_t e = cudaSetDevice(h->device);
-    if (e == cudaSuccess && !h->d_pf) e = cudaMalloc(&h->d_pf, sizeof(DmParseFmt));
-    if (e == cudaSuccess && !h->d_pfmt) e = cudaMalloc(&h->d_pfmt, sizeof(DmFormat));
-    if (e == cudaSuccess && !h->h_ptotal) e = cudaHostAlloc(&h->h_ptotal, sizeof(unsigned long long), cudaHostAllocDefault);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->last_stream);
-    if (e == cudaSuccess) e = cudaMemcpy(h->d_pf, P, sizeof(DmParseFmt), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(h->d_pfmt, pf, sizeof(DmFormat), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = h->h_ptotal.alloc(1);
+    if (e == cudaSuccess) e = dm_upload(h->d_pf, *P, h->last_stream);
+    if (e == cudaSuccess) e = dm_upload(h->d_pfmt, *pf, h->last_stream);
     if (e == cudaSuccess) h->pfmt_slots = pf->max_slots;
-    delete P;
-    delete pf;
     if (e != cudaSuccess) return dm_fail(DM_ERR_CUDA, "dm_set_parser_format: %s", cudaGetErrorString(e));
     h->parse_set = true;
     return DM_OK;
@@ -1152,7 +1083,7 @@ extern "C" int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, 
     if (nbytes && !buf) return dm_fail(DM_ERR_ARG, "buf is NULL");
     if (!h->parse_set) return dm_fail(DM_ERR_STATE, "dm_set_parser_format has not been called since the last dm_set_format");
     if (nbytes > h->max_batch_bytes) return dm_fail(DM_ERR_CAPACITY, "message of %llu bytes exceeds max_batch_bytes=%llu", (unsigned long long)nbytes, (unsigned long long)h->max_batch_bytes);
-    *out = h->h_pout;
+    *out = h->h_pout.get();
     *out_len = 0;
     DmFrames fr;
     int rc = dm_logs_frames(h, buf, nbytes, delimited, &fr);
@@ -1164,22 +1095,17 @@ extern "C" int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, 
     uint8_t* rflags;
     rc = dm_logs_unwrap(h, buf, nbytes, fr, 0, false, &la, &rscores, &rflags);
     if (rc != DM_OK) return rc;
-    cudaStream_t st = h->stream;
+    cudaStream_t st = h->stream.get();
     const uint64_t words = dm_parse_scratch(nullptr, n_records, nullptr, nullptr, nullptr);
-    if (words > h->psize_cap) {
+    if (words > h->d_psize.cap()) {
         DM_CUDA(cudaStreamSynchronize(st));
-        cudaFree(h->d_psize);
-        h->d_psize = nullptr;
-        h->psize_cap = 0;
-        const uint64_t cap = std::max<uint64_t>(2 * words, 8192);
-        DM_CUDA(cudaMalloc(&h->d_psize, cap * sizeof(unsigned long long)));
-        h->psize_cap = cap;
+        DM_CUDA(h->d_psize.grow(words, std::max<uint64_t>(2 * words, 8192)));
     }
-    DmParseArgs a = dm_parse_args(la, h->d_pf, h->d_pfmt, h->d_norm, first_parsed_id, now);
+    DmParseArgs a = dm_parse_args(la, h->d_pf.get(), h->d_pfmt.get(), h->d_norm.get(), first_parsed_id, now);
     unsigned long long *tile_sums, *d_total;
-    dm_parse_scratch(h->d_psize, n_records, &a, &tile_sums, &d_total);
+    dm_parse_scratch(h->d_psize.get(), n_records, &a, &tile_sums, &d_total);
     const bool norm = h->fmt_norm;
-    if (norm && !h->d_norm) return dm_fail(DM_ERR_STATE, "no R-norm scratch");
+    if (norm && !h->d_norm.get()) return dm_fail(DM_ERR_STATE, "no R-norm scratch");
     const size_t smem = (size_t)2 * h->pfmt_slots * DM_FMTL_THREADS * sizeof(uint2);
     const unsigned grid = dm_grid(n_records, DM_FMTL_THREADS, (uint64_t)h->sm_count * 32);
     DM_CUDA(cudaMemsetAsync(d_total, 0, sizeof(unsigned long long), st));
@@ -1189,30 +1115,29 @@ extern "C" int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, 
         h->launches += 4;
         DM_CUDA(cudaGetLastError());
     }
-    DM_CUDA(cudaMemcpyAsync(h->h_ptotal, d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_ptotal.get(), d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
-    const uint64_t total = *h->h_ptotal, n_emitted = h->h_lhdr->n_lines;
-    const uint64_t cap = dm_grow_cap(h->pout_cap, total);
-    if (cap != h->pout_cap) {
-        cudaFree(h->d_pout);
-        cudaFreeHost(h->h_pout);
-        h->d_pout = nullptr;
-        h->h_pout = nullptr;
-        h->pout_cap = 0;
+    const uint64_t total = *h->h_ptotal.get(), n_emitted = h->h_lhdr.get()->n_lines;
+    const uint64_t cap = dm_grow_cap(h->d_pout.cap(), total);
+    if (cap != h->d_pout.cap()) {                              // (both or neither: the old pair is freed first)
         *out = nullptr;
-        DM_CUDA(cudaMalloc(&h->d_pout, cap));
-        DM_CUDA(cudaHostAlloc(&h->h_pout, cap, cudaHostAllocDefault));
-        h->pout_cap = cap;
+        h->d_pout.reset();
+        h->h_pout.reset();
+        DmDev<uint8_t> d_pout; DmPinned<uint8_t> h_pout;
+        DM_CUDA(d_pout.alloc(cap));
+        DM_CUDA(h_pout.alloc(cap));
+        h->d_pout = std::move(d_pout);
+        h->h_pout = std::move(h_pout);
     }
     if (total) {
-        a.out = h->d_pout; a.out_cap = h->pout_cap;
+        a.out = h->d_pout.get(); a.out_cap = h->d_pout.cap();
         dm_parse_kernel(norm, true)<<<grid, DM_FMTL_THREADS, smem, st>>>(a);
         h->launches++;
         DM_CUDA(cudaGetLastError());
-        DM_CUDA(cudaMemcpyAsync(h->h_pout, h->d_pout, total, cudaMemcpyDeviceToHost, st));
+        DM_CUDA(cudaMemcpyAsync(h->h_pout.get(), h->d_pout.get(), total, cudaMemcpyDeviceToHost, st));
         DM_CUDA(cudaStreamSynchronize(st));
     }
-    *out = h->h_pout;
+    *out = h->h_pout.get();
     *out_len = total;
     if (n_records_out) *n_records_out = n_records;
     if (n_emitted_out) *n_emitted_out = n_emitted;
@@ -1222,22 +1147,22 @@ extern "C" int dm_parse_logs(dm_handle* h, const uint8_t* buf, uint64_t nbytes, 
 
 static int dm_slots_init(dm_handle* h) {
     if (h->slots_ready) return DM_OK;
-    DM_CUDA(cudaStreamCreateWithFlags(&h->st_in, cudaStreamNonBlocking));
-    for (auto& sl : h->slots) {
-        DM_CUDA(cudaMalloc(&sl.d_in, h->max_batch_bytes + 256));
-        DM_CUDA(cudaMemset(sl.d_in, 0, h->max_batch_bytes + 256));
-        DM_CUDA(cudaMalloc(&sl.d_flags, h->max_lines + 16));
-        DM_CUDA(cudaMalloc(&sl.d_scores, (h->max_lines + 4) * sizeof(float)));
-        DM_CUDA(cudaMalloc(&sl.d_hdr, sizeof(DmBatchHeader)));
-        DM_CUDA(cudaMemset(sl.d_hdr, 0, sizeof(DmBatchHeader)));
-        DM_CUDA(cudaMalloc(&sl.d_anoms, (uint64_t)h->anomaly_cap * sizeof(dm_anomaly_t)));
-        DM_CUDA(cudaHostAlloc(&sl.h_hdr, sizeof(DmBatchHeader), cudaHostAllocDefault));
-        DM_CUDA(cudaHostAlloc(&sl.h_flags, h->max_lines + 16, cudaHostAllocDefault));
-        DM_CUDA(cudaHostAlloc(&sl.h_scores, (h->max_lines + 4) * sizeof(float), cudaHostAllocDefault));
-        DM_CUDA(cudaEventCreateWithFlags(&sl.ev_in, cudaEventDisableTiming));
-        DM_CUDA(cudaEventCreateWithFlags(&sl.ev_comp, cudaEventDisableTiming));
-        DM_CUDA(cudaEventCreateWithFlags(&sl.ev_hdr, cudaEventDisableTiming));
-        DM_CUDA(cudaStreamCreateWithFlags(&sl.st_out, cudaStreamNonBlocking));
+    DM_CUDA(h->st_in.create());
+    for (auto& slot : h->slots) {
+        dm_handle::Slot sl;                                    // (kept only when all of it was created)
+        DM_CUDA(sl.d_in.alloc(h->max_batch_bytes + 256, true));
+        DM_CUDA(sl.d_flags.alloc(h->max_lines + 16));
+        DM_CUDA(sl.d_scores.alloc(h->max_lines + 4));
+        DM_CUDA(sl.d_hdr.alloc(1, true));
+        DM_CUDA(sl.d_anoms.alloc(h->anomaly_cap));
+        DM_CUDA(sl.h_hdr.alloc(1));
+        DM_CUDA(sl.h_flags.alloc(h->max_lines + 16));
+        DM_CUDA(sl.h_scores.alloc(h->max_lines + 4));
+        DM_CUDA(sl.ev_in.create());
+        DM_CUDA(sl.ev_comp.create());
+        DM_CUDA(sl.ev_hdr.create());
+        DM_CUDA(sl.st_out.create());
+        slot = std::move(sl);
     }
     h->slots_ready = true;
     return DM_OK;
@@ -1257,24 +1182,24 @@ extern "C" int dm_submit_lines(dm_handle* h, const uint8_t* host_buf, uint64_t n
     if (rc != DM_OK) return rc;
     dm_handle::Slot& sl = h->slots[slot];
     if (sl.busy) return dm_fail(DM_ERR_STATE, "slot %u was submitted and not collected yet", slot);
-    if (nbytes) DM_CUDA(cudaMemcpyAsync(sl.d_in, host_buf, nbytes, cudaMemcpyHostToDevice, h->st_in));
-    DM_CUDA(cudaMemsetAsync(sl.d_in + nbytes, 0, 64, h->st_in));
+    if (nbytes) DM_CUDA(cudaMemcpyAsync(sl.d_in.get(), host_buf, nbytes, cudaMemcpyHostToDevice, h->st_in.get()));
+    DM_CUDA(cudaMemsetAsync(sl.d_in.get() + nbytes, 0, 64, h->st_in.get()));
     h->slot_nbytes[slot] = nbytes;
-    DM_CUDA(cudaEventRecord(sl.ev_in, h->st_in));
-    cudaStream_t st = h->stream;                       // ONE compute stream: submission order = processing order
+    DM_CUDA(cudaEventRecord(sl.ev_in.get(), h->st_in.get()));
+    cudaStream_t st = h->stream.get();                       // ONE compute stream: submission order = processing order
     rc = dm_use_stream(h, st);
     if (rc != DM_OK) return rc;
     h->last_src = DMA_SRC_NONE;
-    DM_CUDA(cudaStreamWaitEvent(st, sl.ev_in, 0));
-    if (nbytes == 0) DM_CUDA(cudaMemsetAsync(sl.d_hdr, 0, sizeof(DmBatchHeader), st));
-    const int launched = dmx_launch(&h->dmx, sl.d_in, nbytes, n_train_lines, h->table, sl.d_flags, sl.d_scores, h->max_lines, sl.d_anoms,
-                                    h->anomaly_cap, sl.d_hdr, h->d_stats, h->max_lines, st, true, false, dm_prof_mark_cb, h);
+    DM_CUDA(cudaStreamWaitEvent(st, sl.ev_in.get(), 0));
+    if (nbytes == 0) DM_CUDA(cudaMemsetAsync(sl.d_hdr.get(), 0, sizeof(DmBatchHeader), st));
+    const int launched = dmx_launch(&h->dmx, sl.d_in.get(), nbytes, n_train_lines, h->table, sl.d_flags.get(), sl.d_scores.get(), h->max_lines, sl.d_anoms.get(),
+                                    h->anomaly_cap, sl.d_hdr.get(), h->d_stats.get(), h->max_lines, st, true, false, dm_prof_mark_cb, h);
     if (launched < 0) return dm_fail(DM_ERR_CUDA, "stream kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     h->launches += (uint64_t)launched;
-    DM_CUDA(cudaEventRecord(sl.ev_comp, st));
-    DM_CUDA(cudaStreamWaitEvent(sl.st_out, sl.ev_comp, 0));
-    DM_CUDA(cudaMemcpyAsync(sl.h_hdr, sl.d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, sl.st_out));
-    DM_CUDA(cudaEventRecord(sl.ev_hdr, sl.st_out));
+    DM_CUDA(cudaEventRecord(sl.ev_comp.get(), st));
+    DM_CUDA(cudaStreamWaitEvent(sl.st_out.get(), sl.ev_comp.get(), 0));
+    DM_CUDA(cudaMemcpyAsync(sl.h_hdr.get(), sl.d_hdr.get(), sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, sl.st_out.get()));
+    DM_CUDA(cudaEventRecord(sl.ev_hdr.get(), sl.st_out.get()));
     sl.busy = true;
     return DM_OK;
 }
@@ -1285,25 +1210,25 @@ extern "C" int dm_collect(dm_handle* h, uint32_t slot, const uint8_t** flags_out
     if (slot > 1 || !h->slots_ready || !h->slots[slot].busy) return dm_fail(DM_ERR_STATE, "slot %u has nothing to collect", slot);
     DM_CUDA(cudaSetDevice(h->device));
     dm_handle::Slot& sl = h->slots[slot];
-    DM_CUDA(cudaEventSynchronize(sl.ev_hdr));
+    DM_CUDA(cudaEventSynchronize(sl.ev_hdr.get()));
     sl.busy = false;
-    *h->h_hdr = *sl.h_hdr;
+    *h->h_hdr.get() = *sl.h_hdr.get();
     int rc = dm_check_device_errors(h);
     if (rc != DM_OK) return rc;
-    const uint64_t n = sl.h_hdr->n_lines;
+    const uint64_t n = sl.h_hdr.get()->n_lines;
     if (n && (flags_out || scores_out)) {
-        if (flags_out) DM_CUDA(cudaMemcpyAsync(sl.h_flags, sl.d_flags, n, cudaMemcpyDeviceToHost, sl.st_out));
-        if (scores_out) DM_CUDA(cudaMemcpyAsync(sl.h_scores, sl.d_scores, n * sizeof(float), cudaMemcpyDeviceToHost, sl.st_out));
-        DM_CUDA(cudaStreamSynchronize(sl.st_out));
+        if (flags_out) DM_CUDA(cudaMemcpyAsync(sl.h_flags.get(), sl.d_flags.get(), n, cudaMemcpyDeviceToHost, sl.st_out.get()));
+        if (scores_out) DM_CUDA(cudaMemcpyAsync(sl.h_scores.get(), sl.d_scores.get(), n * sizeof(float), cudaMemcpyDeviceToHost, sl.st_out.get()));
+        DM_CUDA(cudaStreamSynchronize(sl.st_out.get()));
     }
-    if (flags_out) *flags_out = sl.h_flags;
-    if (scores_out) *scores_out = sl.h_scores;
+    if (flags_out) *flags_out = sl.h_flags.get();
+    if (scores_out) *scores_out = sl.h_scores.get();
     if (n_lines_out) *n_lines_out = n;
-    if (n_anomalies_out) *n_anomalies_out = sl.h_hdr->n_anomalies;
+    if (n_anomalies_out) *n_anomalies_out = sl.h_hdr.get()->n_anomalies;
     // the slot's batch is now the last batch, for dm_encode_alerts
-    h->last_buf = sl.d_in;
+    h->last_buf = sl.d_in.get();
     h->last_nbytes = h->slot_nbytes[slot];
-    h->last_scores = sl.d_scores;
+    h->last_scores = sl.d_scores.get();
     h->last_src = DMA_LINES;
     h->last_slot = (int)slot;
     return DM_OK;
@@ -1329,21 +1254,21 @@ extern "C" int dm_collect_anomalies(dm_handle* h, uint32_t slot, dm_anomaly_t* o
     DM_CUDA(cudaSetDevice(h->device));
     dm_handle::Slot& sl = h->slots[slot];
     if (sl.busy) return dm_fail(DM_ERR_STATE, "slot %u is still in flight: dm_collect it first", slot);
-    return dm_fetch_anomalies(h, sl.d_anoms, sl.h_hdr->anomaly_list_count, out, cap, n_out);
+    return dm_fetch_anomalies(h, sl.d_anoms.get(), sl.h_hdr.get()->anomaly_list_count, out, cap, n_out);
 }
 
 extern "C" int dm_sync(dm_handle* h, uint64_t* n_lines_out, uint64_t* n_anomalies_out) {
     if (!h) return dm_fail(DM_ERR_ARG, "handle is NULL");
     DM_CUDA(cudaSetDevice(h->device));
-    DM_CUDA(cudaStreamWaitEvent(h->last_stream, h->ev_import, 0));     // the last window import, whatever its stream
-    DM_CUDA(cudaMemcpyAsync(h->h_hdr, h->d_hdr, sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, h->last_stream));
+    DM_CUDA(cudaStreamWaitEvent(h->last_stream, h->ev_import.get(), 0));     // the last window import, whatever its stream
+    DM_CUDA(cudaMemcpyAsync(h->h_hdr.get(), h->d_hdr.get(), sizeof(DmBatchHeader), cudaMemcpyDeviceToHost, h->last_stream));
     int rc = dm_fetch_errors(h, h->last_stream);
     if (rc != DM_OK) return rc;
     DM_CUDA(cudaStreamSynchronize(h->last_stream));
     rc = dm_header_with_errors(h);
     if (rc != DM_OK) return rc;
-    if (n_lines_out) *n_lines_out = h->h_hdr->n_lines;
-    if (n_anomalies_out) *n_anomalies_out = h->h_hdr->n_anomalies;
+    if (n_lines_out) *n_lines_out = h->h_hdr.get()->n_lines;
+    if (n_anomalies_out) *n_anomalies_out = h->h_hdr.get()->n_anomalies;
     return DM_OK;
 }
 
@@ -1352,10 +1277,10 @@ extern "C" int dm_get_anomalies(dm_handle* h, dm_anomaly_t* out, uint32_t cap, u
     DM_CUDA(cudaSetDevice(h->device));
     int rc = dm_sync(h, nullptr, nullptr);
     if (rc != DM_OK) return rc;
-    const uint32_t total = h->h_hdr->anomaly_list_count;
-    *n_out = std::min<uint64_t>(total, h->h_hdr->n_anomalies ? h->h_hdr->n_anomalies : total);
+    const uint32_t total = h->h_hdr.get()->anomaly_list_count;
+    *n_out = std::min<uint64_t>(total, h->h_hdr.get()->n_anomalies ? h->h_hdr.get()->n_anomalies : total);
     if (!out || cap == 0 || std::min(total, h->anomaly_cap) == 0) return DM_OK;
-    return dm_fetch_anomalies(h, h->d_anoms, total, out, cap, n_out);
+    return dm_fetch_anomalies(h, h->d_anoms.get(), total, out, cap, n_out);
 }
 
 static void dm_words_to_stats(const unsigned long long* w, dm_stats_t* out) {
@@ -1368,8 +1293,8 @@ extern "C" int dm_get_stats(dm_handle* h, dm_stats_t* out) {
     if (!h || !out) return dm_fail(DM_ERR_ARG, "NULL argument");
     DM_CUDA(cudaSetDevice(h->device));
     DM_CUDA(cudaStreamSynchronize(h->last_stream));
-    DM_CUDA(cudaMemcpy(h->h_stats, h->d_stats, DM_STATS_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    dm_words_to_stats(h->h_stats, out);
+    DM_CUDA(cudaMemcpy(h->h_stats.get(), h->d_stats.get(), DM_STATS_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    dm_words_to_stats(h->h_stats.get(), out);
     unsigned long long cnt = 0;
     DM_CUDA(cudaMemcpy(&cnt, h->table.count, sizeof(cnt), cudaMemcpyDeviceToHost));
     out->known_keys = cnt;
@@ -1379,10 +1304,10 @@ extern "C" int dm_get_stats(dm_handle* h, dm_stats_t* out) {
 extern "C" int dm_get_global_stats(dm_handle* h, dm_stats_t* out) {
     if (!h || !out) return dm_fail(DM_ERR_ARG, "NULL argument");
     DM_CUDA(cudaSetDevice(h->device));
-    DM_CUDA(cudaStreamWaitEvent(h->last_stream, h->ev_import, 0));     // the last window import, whatever its stream
+    DM_CUDA(cudaStreamWaitEvent(h->last_stream, h->ev_import.get(), 0));     // the last window import, whatever its stream
     DM_CUDA(cudaStreamSynchronize(h->last_stream));
-    DM_CUDA(cudaMemcpy(h->h_stats, h->d_stats_global, DM_STATS_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    dm_words_to_stats(h->h_stats, out);
+    DM_CUDA(cudaMemcpy(h->h_stats.get(), h->d_stats_global, DM_STATS_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    dm_words_to_stats(h->h_stats.get(), out);
     return DM_OK;
 }
 
@@ -1404,16 +1329,17 @@ extern "C" int dm_export_known(dm_handle* h, uint64_t* keys_out, uint64_t cap, u
     // the scratch holds the load limit's slots/2 keys; only a table filled past its limit (its training reported
     // DM_ERR_TABLE_FULL) holds more, and then the scratch grows once to its count
     const uint64_t slots = (uint64_t)h->table.mask + 1;
-    if (h->known.kcap < n) {
-        cudaFree(h->known_buf);
-        cudaFreeHost(h->h_known_hist);
-        h->known_buf = nullptr;
-        h->h_known_hist = nullptr;
-        h->known.kcap = 0;
+    if (h->known.kcap < n) {                                   // (both or neither: the old pair is freed first)
+        h->known = DmKnownScratch{};
+        h->known_buf.reset();
+        h->h_known_hist.reset();
         const uint64_t kcap = std::max<uint64_t>(n, slots / 2);
-        DM_CUDA(cudaMalloc(&h->known_buf, dm_known_scratch(nullptr, kcap, nullptr)));
-        DM_CUDA(cudaHostAlloc(&h->h_known_hist, DMK_HIST_WORDS * sizeof(unsigned int), cudaHostAllocDefault));
-        dm_known_scratch(h->known_buf, kcap, &h->known);
+        DmDev<uint8_t> buf; DmPinned<unsigned int> hist;
+        DM_CUDA(buf.alloc(dm_known_scratch(nullptr, kcap, nullptr)));
+        DM_CUDA(hist.alloc(DMK_HIST_WORDS));
+        h->known_buf = std::move(buf);
+        h->h_known_hist = std::move(hist);
+        dm_known_scratch(h->known_buf.get(), kcap, &h->known);
     }
     DmKnownScratch& s = h->known;
     DM_CUDA(cudaMemsetAsync(s.hist, 0, DMK_HIST_WORDS * sizeof(unsigned int), st));
@@ -1421,12 +1347,12 @@ extern "C" int dm_export_known(dm_handle* h, uint64_t* keys_out, uint64_t cap, u
         h->table.slots, slots, s.a, s.kcap, s.hist + DMK_PASSES * DMK_BINS);
     dm_k_known_digits<<<dm_grid(n, DMK_THREADS * 16, 2 * (uint64_t)h->sm_count), DMK_THREADS, 0, st>>>(s.a, n, s.hist);
     DM_CUDA(cudaGetLastError());
-    DM_CUDA(cudaMemcpyAsync(h->h_known_hist, s.hist, DMK_HIST_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+    DM_CUDA(cudaMemcpyAsync(h->h_known_hist.get(), s.hist, DMK_HIST_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
     DM_CUDA(cudaStreamSynchronize(st));
-    if (h->h_known_hist[DMK_PASSES * DMK_BINS] != n)
-        return dm_fail(DM_ERR_STATE, "the table holds %u keys, its count says %llu", h->h_known_hist[DMK_PASSES * DMK_BINS], n);
+    if (h->h_known_hist.get()[DMK_PASSES * DMK_BINS] != n)
+        return dm_fail(DM_ERR_STATE, "the table holds %u keys, its count says %llu", h->h_known_hist.get()[DMK_PASSES * DMK_BINS], n);
     uint32_t shifts[DMK_PASSES];
-    const uint32_t n_passes = dm_known_passes(h->h_known_hist, n, shifts);
+    const uint32_t n_passes = dm_known_passes(h->h_known_hist.get(), n, shifts);
     const uint32_t tiles = (uint32_t)dm_known_tiles(n);
     unsigned long long *src = s.a, *dst = s.b;
     for (uint32_t p = 0; p < n_passes; ++p) {
@@ -1445,17 +1371,15 @@ extern "C" int dm_import_known(dm_handle* h, const uint64_t* keys, uint64_t n) {
     if (!h || (n && !keys)) return dm_fail(DM_ERR_ARG, "NULL argument");
     if (n == 0) return DM_OK;
     DM_CUDA(cudaSetDevice(h->device));
-    unsigned long long* d_tmp = nullptr;
-    DM_CUDA(cudaMalloc(&d_tmp, n * sizeof(unsigned long long)));
-    DM_CUDA(cudaMemcpy(d_tmp, keys, n * sizeof(unsigned long long), cudaMemcpyHostToDevice));
-    DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), h->last_stream));
+    DmDev<unsigned long long> d_tmp;
+    DM_CUDA(d_tmp.alloc(n));
+    DM_CUDA(cudaMemcpy(d_tmp.get(), keys, n * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+    DM_CUDA(cudaMemsetAsync(h->d_hdr.get(), 0, sizeof(DmBatchHeader), h->last_stream));
     dm_break_chain(h, h->last_stream);
     h->last_src = DMA_SRC_NONE;
-    dm_k_insert_keys<<<std::max(1, (int)std::min<uint64_t>((n + 255) / 256, 1024)), 256, 0, h->last_stream>>>(h->table, d_tmp, n, &h->d_hdr->error);
+    dm_k_insert_keys<<<std::max(1, (int)std::min<uint64_t>((n + 255) / 256, 1024)), 256, 0, h->last_stream>>>(h->table, d_tmp.get(), n, &h->d_hdr.get()->error);
     DM_CUDA(cudaGetLastError());
-    int rc = dm_sync(h, nullptr, nullptr);
-    cudaFree(d_tmp);
-    return rc;
+    return dm_sync(h, nullptr, nullptr);
 }
 
 extern "C" int dm_reset(dm_handle* h) {
@@ -1467,8 +1391,8 @@ extern "C" int dm_reset(dm_handle* h) {
     dm_break_chain(h, st);
     DM_CUDA(cudaMemsetAsync(h->table.slots, 0, ((uint64_t)h->table.mask + 1) * sizeof(unsigned long long), st));
     DM_CUDA(cudaMemsetAsync(h->table.count, 0, 2 * sizeof(unsigned long long), st));
-    DM_CUDA(cudaMemsetAsync(h->d_stats, 0, 3 * DM_STATS_WORDS * sizeof(unsigned long long), st));
-    DM_CUDA(cudaMemsetAsync(h->d_hdr, 0, sizeof(DmBatchHeader), st));
+    DM_CUDA(cudaMemsetAsync(h->d_stats.get(), 0, 3 * DM_STATS_WORDS * sizeof(unsigned long long), st));
+    DM_CUDA(cudaMemsetAsync(h->d_hdr.get(), 0, sizeof(DmBatchHeader), st));
     DM_CUDA(cudaStreamSynchronize(st));
     h->novel_exported = 0;
     h->novel_pending = 0;
@@ -1487,7 +1411,7 @@ extern "C" uint64_t dm_window_words(dm_handle* h, uint32_t world, int with_keys)
 extern "C" int dm_window_export(dm_handle* h, uint64_t* dev_buf, uint32_t rank, uint32_t world, int with_keys, void* stream_) {
     if (!h || !dev_buf || rank >= world) return dm_fail(DM_ERR_ARG, "bad window arguments");
     DM_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream;     // (not recorded as the compute stream)
+    cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream.get();     // (not recorded as the compute stream)
     dm_break_chain(h, st);
     DmWindowKeys wk{h->novel_exported, h->novel_exported, 0};
     if (with_keys) {
@@ -1503,7 +1427,7 @@ extern "C" int dm_window_export(dm_handle* h, uint64_t* dev_buf, uint32_t rank, 
     const uint64_t n_words = dm_window_words(h, world, with_keys);
     const uint64_t seg_off = dm_window_n_words(rank, true, DM_WINDOW_KEYS);
     dm_k_window_export<<<std::max(1, (int)std::min<uint64_t>((n_words + 255) / 256, 2048)), 256, 0, st>>>(
-        (unsigned long long*)dev_buf, n_words, h->d_stats, h->d_stats_exported, h->table.novel, wk.from, wk.to, seg_off,
+        (unsigned long long*)dev_buf, n_words, h->d_stats.get(), h->d_stats_exported, h->table.novel, wk.from, wk.to, seg_off,
         DM_WINDOW_KEYS, with_keys);
     DM_CUDA(cudaGetLastError());
     h->novel_exported = wk.to;
@@ -1519,14 +1443,14 @@ extern "C" int dm_window_pending_keys(dm_handle* h, uint64_t* n_out) {
 extern "C" int dm_window_import(dm_handle* h, const uint64_t* dev_buf, uint32_t rank, uint32_t world, int with_keys, void* stream_) {
     if (!h || !dev_buf || rank >= world) return dm_fail(DM_ERR_ARG, "bad window arguments");
     DM_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream;     // (not recorded as the compute stream)
+    cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream.get();     // (not recorded as the compute stream)
     dm_break_chain(h, st);
     // errors go to the handle's accumulating error word, which no launch overwrites: the next dm_sync or synchronous
     // dm_process_lines reports them (the batch header's word is rewritten by the next detection launch)
     dm_k_window_import<<<with_keys ? 256 : 1, 256, 0, st>>>((const unsigned long long*)dev_buf, world, rank, DM_WINDOW_KEYS,
-                                                          h->d_stats_global, h->table, &h->dmx.d_shared->error, with_keys);
+                                                          h->d_stats_global, h->table, &h->dmx.d_shared.get()->error, with_keys);
     DM_CUDA(cudaGetLastError());
-    DM_CUDA(cudaEventRecord(h->ev_import, st));     // dm_sync and dm_get_global_stats wait for it
+    DM_CUDA(cudaEventRecord(h->ev_import.get(), st));     // dm_sync and dm_get_global_stats wait for it
     return DM_OK;
 }
 
@@ -1602,8 +1526,8 @@ extern "C" int dm_nccl_init(dm_handle* h, const uint8_t* ids, uint32_t n_comms, 
         const int r = g_nccl.init_rank(&comm, (int)world, id, (int)rank);
         if (r != 0) return dm_fail(DM_ERR_CUDA, "ncclCommInitRank: %s", g_nccl.err(r));
         h->nccl_comm[k] = comm;
-        DM_CUDA(cudaMalloc(&h->d_win[k], dm_window_words(h, world, 1) * sizeof(unsigned long long)));
-        DM_CUDA(cudaEventCreateWithFlags(&h->ev_win_done[k], cudaEventDisableTiming));
+        DM_CUDA(h->d_win[k].alloc(dm_window_words(h, world, 1)));
+        DM_CUDA(h->ev_win_done[k].create());
     }
     h->nccl_n = n_comms; h->nccl_rank = rank; h->nccl_world = world;
     return DM_OK;
@@ -1616,17 +1540,17 @@ extern "C" int dm_window_allreduce(dm_handle* h, int with_keys, void* stream_) {
     // alternating streams, two all-reduces are in flight, which matters at 8 ranks where one
     // export + all-reduce + import chain is longer than a step
     const uint32_t k = (uint32_t)(h->win_seq++ % h->nccl_n);
-    cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream;     // (not recorded as the compute stream)
+    cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream.get();     // (not recorded as the compute stream)
     DM_CUDA(cudaSetDevice(h->device));
-    DM_CUDA(cudaStreamWaitEvent(st, h->ev_win_done[k], 0));           // the buffer's previous window is through
-    int rc = dm_window_export(h, (uint64_t*)h->d_win[k], h->nccl_rank, h->nccl_world, with_keys, stream_);
+    DM_CUDA(cudaStreamWaitEvent(st, h->ev_win_done[k].get(), 0));           // the buffer's previous window is through
+    int rc = dm_window_export(h, (uint64_t*)h->d_win[k].get(), h->nccl_rank, h->nccl_world, with_keys, stream_);
     if (rc != DM_OK) return rc;
-    const int r = g_nccl.all_reduce(h->d_win[k], h->d_win[k], (size_t)dm_window_words(h, h->nccl_world, with_keys),
+    const int r = g_nccl.all_reduce(h->d_win[k].get(), h->d_win[k].get(), (size_t)dm_window_words(h, h->nccl_world, with_keys),
                                     DM_NCCL_UINT64, DM_NCCL_SUM, h->nccl_comm[k], st);
     if (r != 0) return dm_fail(DM_ERR_CUDA, "ncclAllReduce: %s", g_nccl.err(r));
-    rc = dm_window_import(h, (const uint64_t*)h->d_win[k], h->nccl_rank, h->nccl_world, with_keys, stream_);
+    rc = dm_window_import(h, (const uint64_t*)h->d_win[k].get(), h->nccl_rank, h->nccl_world, with_keys, stream_);
     if (rc != DM_OK) return rc;
-    DM_CUDA(cudaEventRecord(h->ev_win_done[k], st));
+    DM_CUDA(cudaEventRecord(h->ev_win_done[k].get(), st));
     return DM_OK;
 }
 

@@ -17,7 +17,8 @@
  *   - one handle = one device = one caller thread at a time (the reference calls process()
  *     from the single EngineLoop thread only, engine.py:80-82).
  *   - the caller owns every buffer it passes in; the library owns its tables and scratch
- *     (allocated once in dm_create, no per-call cudaMalloc).
+ *     (allocated in dm_create or on first use, and grown when a batch needs more;
+ *     dm_import_known stages the keys it is given in a buffer of its own).
  *   - there is NO CPU fallback: without a usable CUDA device dm_create fails.
  */
 #ifndef DMDETECT_H
